@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark of the HAWQ integer forward path on B200 (contract in the task statement / DESIGN.md §Measurement).
+"""Benchmark of the HAWQ integer forward path on H100 (DESIGN.md §Measurement).
 
   python bench.py --gpus N --steps K --warmup W            one JSON line: images/s of the quantized ResNet forward
   python bench.py --impl reference ...                     the reference's CPU path (oracle port) on the host cores
+  python bench.py ... --dump-outputs DIR                   also write the logits of the last timed step to DIR/logits.npy
 
 A "step" = one forward of the frozen quantized ResNet over one batch of synthetic int8 images per GPU.
 Default workload: ResNet-50 W8A8 (bit_config_resnet50_uniform8), batch 128 per GPU (BASELINE.json configs[2]).
@@ -21,9 +22,9 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
-METRIC = "images/sec ResNet-50 W8A8 & W4A4 @batch128, 1/2/4/8xB200; % int-TC roofline"
+METRIC = "images/sec ResNet-50 W8A8 & W4A4 @batch128, 1/2/4/8xH100; % int-TC roofline"
 MACS_PER_IMAGE = {"resnet18": 1.8141e9, "resnet50": 3.8580e9, "resnet101": 7.57e9}
-INT8_TC_PEAK_OPS = 4.5e15        # nominal dense int8 tcgen05 peak (op/s); reported for context only
+INT8_TC_PEAK_OPS = 1.979e15      # H100 SXM data-sheet dense int8 tensor-core peak at 700 W (op/s); reported for context only
 
 
 def parse():
@@ -43,6 +44,8 @@ def parse():
     ap.add_argument("--a4-storage", default="byte", choices=["byte", "packed"],
                     help="HBM container of 4-bit activations: one value per byte (default, consumed directly by the int8 tensor-core kernels) or packed nibbles expanded on chip")
     ap.add_argument("--detail", default="", help="write per-layer timings to this JSON file")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the float32 logits of the last timed step to DIR/logits.npy (inputs are seeded: runs with the same arguments compare)")
     return ap.parse_args()
 
 
@@ -52,7 +55,7 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured", d
-    return 6650.0, "fallback", {}
+    return 3350.0, "fallback", {}
 
 
 # ----------------------------------------------------------------------------------------------- clocks
@@ -152,9 +155,8 @@ def cpu_forward_rate(arch, scheme, max_batch, steps, warmup, budget_s=25.0, fixe
     t0 = time.perf_counter()
     m(x1)
     per_img = time.perf_counter() - t0
-    if fixed_batch:      # every step is a full batch of the workload; the budget bounds the number of steps (>= 1)
+    if fixed_batch:      # every step is a full batch of the workload; exactly `steps` steps are timed
         batch = max_batch
-        steps = max(1, min(steps, int(budget_s / max(per_img * batch * 0.8, 1e-6)) - 1))
     else:
         steps = max(1, min(steps, int(4 * budget_s / max(per_img, 1e-6))))   # a pathologically slow host: fewer steps rather than minutes
         batch = int(max(1, min(max_batch, budget_s / max(steps, 1) / max(per_img, 1e-6))))
@@ -172,22 +174,21 @@ def cpu_forward_rate(arch, scheme, max_batch, steps, warmup, budget_s=25.0, fixe
 
 def run_reference(a):
     """The reference's CPU path on this box's host cores, on OUR arm's workload: every step is one forward of a.batch images
-    (the configuration our JSON line names).  The number of timed steps is bounded by a time budget (a batch-128 ResNet-50
-    forward takes ~13 s on 16 cores), and the line says how many ran."""
+    (the configuration our JSON line names), exactly --steps timed steps (a batch-128 ResNet-50 forward takes ~13 s on 16 cores)."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
     steps = max(1, a.steps)
     warm = max(1, a.warmup)
-    ips, threads, sec, cpu_b, steps = cpu_forward_rate(a.arch, a.scheme, a.batch, steps, warm, budget_s=120.0, fixed_batch=True)
+    ips, threads, sec, cpu_b, steps = cpu_forward_rate(a.arch, a.scheme, a.batch, steps, warm, fixed_batch=True)
     line = {"metric": METRIC, "value": ips, "unit": "images/s", "n_gpus": a.gpus, "steps": steps, "warmup": 1,
             "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "fp32 emulating int8/int4 (reference fake-quant)", "data": "synthetic", "impl": "reference",
             "config": workload_config(a, 1, None),
             "cpu_baseline": {"value": ips, "unit": "images/s", "cores": threads, "kind": "port",
-                             "sample": "%d timed step(s) (of the %d requested: bounded by a 120 s budget), each the forward of %d images, through oracle/fakequant.py "
+                             "sample": "%d timed step(s), each the forward of %d images, through oracle/fakequant.py "
                                        "(torch CPU restatement of the reference forward, bit-exact vs the unmodified reference in the build container)"
-                                       % (steps, max(1, a.steps), cpu_b)},
+                                       % (steps, cpu_b)},
             "e2e": {"value": ips, "unit": "images/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "gpu_launches": 0}
     print(json.dumps(line))
@@ -269,12 +270,24 @@ def run_ours(a):
     t_begin = time.perf_counter()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    out = None
     for i in range(a.steps):
-        step(i, dev_pool)
+        out = step(i, dev_pool)
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
     flag = int(eng.flag.item())
+    if a.dump_outputs and out is not None:
+        # what a caller receives for the last timed batch: the fast graph's logits, or (uint16 stream overflowed) the exact re-run
+        over = torch.tensor([flag & 1], dtype=torch.int32, device=dev)
+        if world > 1:                      # the exact re-run replays the collective: every rank takes part or none
+            dist.all_reduce(over, op=dist.ReduceOp.MAX)
+        if int(over.item()):
+            out = eng(dev_pool[(a.steps - 1) % POOL])
+        if rank == 0:
+            import numpy as np
+            os.makedirs(a.dump_outputs, exist_ok=True)
+            np.save(os.path.join(a.dump_outputs, "logits.npy"), out.float().cpu().numpy())
     # ---- end-to-end through the public call with host buffers ("e2e")
     # public call: CompiledModel.run_pipelined(host batches) -> host logits; per step it copies the pinned int8 batch H2D,
     # replays the forward, reads logits + status flags back D2H (checked before the result is handed out)
@@ -336,7 +349,7 @@ def run_ours(a):
                                                                 % ("packed nibbles" if a.a4_storage == "packed" else "one per byte")),
                 "data": "synthetic",
                 "config": dict(workload_config(a, world, detail),
-                               l2=("per-step working set (%.1f GB of activations) exceeds the 126 MB L2; %d input batches rotate" % (detail["act_bytes"] / 1e9, POOL)) if detail and detail["act_bytes"] > 2.5e8
+                               l2=("per-step working set (%.1f GB of activations) exceeds the 50 MB L2; %d input batches rotate" % (detail["act_bytes"] / 1e9, POOL)) if detail and detail["act_bytes"] > 1e8
                                else "%d input batches rotate; at this batch size the per-step working set is L2-resident (latency-bound regime)" % POOL,
                                residual_stream="uint%d" % a.residual_bits if a.residual_bits == 16 else "int32", cuda_graph=True,
                                a4_storage=a.a4_storage,
@@ -401,7 +414,8 @@ def small_batch_leg(hb, q, dev, s_in, a, b):
 
 def parity_check(hb, q, eng, x, rank=0):
     """Logits of one timed batch through the benchmarked path vs an eager (un-graphed) run of the same batch with int32
-    residuals and no ratio promises.  Two independent kernel sets (fused tcgen05 / generic IMMA) must agree bit for bit."""
+    residuals and no ratio promises.  Two kernel configurations (fused dual convolution + FP64-FMA requant / generic exact
+    integer requant) must agree bit for bit."""
     from hawq_b200 import qtensor
     from hawq_b200.qtensor import IntActivation, Node
     fast = eng(x).clone()
@@ -411,17 +425,9 @@ def parity_check(hb, q, eng, x, rank=0):
     with torch.no_grad(), qtensor.engine_mode(residual_bits=32, fast_kernels=False, checked=False):
         ref = q(IntActivation(Node("int", (n, c, h, w), data=x.view(-1), bits=8, signed=True), x.device))
     torch.cuda.synchronize()
-    return {"what": "all %d x %d logits of one timed batch: benchmarked path (CUDA graph, fused tcgen05 kernels, uint16 stream) vs eager generic "
+    return {"what": "all %d x %d logits of one timed batch: benchmarked path (CUDA graph, fused dual convolutions, uint16 stream) vs eager generic "
                     "kernels on the int32 stream" % tuple(fast.shape),
             "bit_equal": bool(torch.equal(fast, ref)), "rows_checked": int(fast.shape[0])}
-
-
-def build_digest():
-    from hawq_b200.build import OUT
-    try:
-        return open(OUT + ".stamp").read().strip()[:16]
-    except OSError:
-        return None
 
 
 def roofline_leg(hb, ops, q, dev_pool, a, graph_ms_per_step):
@@ -458,33 +464,16 @@ def roofline_leg(hb, ops, q, dev_pool, a, graph_ms_per_step):
         g["ms"] += ms; g["bytes"] += r["bytes"]; g["macs"] += r["macs"]; g["launches"] += 1
     total_ms = sum(g["ms"] for g in agg.values())
     scale = graph_ms_per_step / total_ms             # eager event time -> time inside the graph-timed step
-    # kernel families: conv_tc (+ its dual-accumulator instantiation) is one template; conv_halo is the in-place 3x3 kernel
-    fam = {}
-    for k, g in agg.items():
-        f = fam.setdefault("conv_tc_kernel" if k.startswith("conv_tc") else ("conv_halo_kernel" if k == "conv_halo" else "conv1x1_kernel" if k == "conv1x1" else "conv_dual_kernel" if k == "conv_dual" else "stem_tc_kernel" if k == "stem_tc" else k),
-                           {"ms": 0.0, "bytes": 0, "macs": 0, "launches": 0})
-        for key in f:
-            f[key] += g[key]
+    fam = agg   # kernel families: the per-launch labels of hawq_b200.ops
     top = max(fam, key=lambda k: fam[k]["ms"])
     t = fam[top]
     achieved = t["bytes"] / (t["ms"] * scale / 1e3) / 1e9
-    # measured DRAM traffic of that kernel: from the ncu pass over this command with THIS build (tools/summarize_ncu.py writes the
-    # build digest next to the numbers); a stale or missing entry gives null
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            ent = json.load(f).get("%s:%s:%d" % (a.arch, a.scheme, a.batch))
-        if ent and ent.get("build") == build_digest() and top in ent.get("kernels", {}):
-            traffic = ent["kernels"][top]["traffic_bytes_per_launch"]
-    except (OSError, ValueError, KeyError):
-        traffic = None
     families = {k: {"launches_per_step": v["launches"], "share_of_step": v["ms"] / total_ms, "ms_in_step": v["ms"] * scale,
                     "algorithmic_GBps": v["bytes"] / (v["ms"] * scale / 1e3) / 1e9, "frac_of_hbm_peak": v["bytes"] / (v["ms"] * scale / 1e3) / 1e9 / peak,
                     "tensor_tops": 2 * v["macs"] / (v["ms"] * scale / 1e3) / 1e12} for k, v in sorted(fam.items(), key=lambda kv: -kv[1]["ms"])}
     step_bytes = sum(g["bytes"] for g in agg.values())
     roof = {"bound": "hbm", "kernel": top, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "peak_source": "%s (MEASURED_PEAKS.json hbm_gbs)" % which if which == "measured" else "fallback 6650 GB/s",
-            "traffic": traffic, "traffic_unit": "bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum, ncu, this build)" if traffic else None,
+            "peak_source": "%s (MEASURED_PEAKS.json hbm_gbs)" % which if which == "measured" else "fallback 3350 GB/s (H100 SXM data sheet)",
             "algorithmic_bytes_per_launch": t["bytes"] / t["launches"],
             "launches_per_step": t["launches"], "share_of_step": t["ms"] / total_ms,
             "algorithmic_bytes_per_step": t["bytes"], "avg_launch_ms": t["ms"] * scale / t["launches"],

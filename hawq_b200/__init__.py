@@ -1,4 +1,4 @@
-"""hawq_b200 — B200-native integer inference engine for HAWQ-quantized ResNets.
+"""hawq_b200 — H100-native integer inference engine for HAWQ-quantized ResNets.
 
 Public surface (mirrors the reference's module API for the quantized forward path):
   modules      QuantAct, QuantBnConv2d, QuantConv2d, QuantLinear, QuantAveragePool2d, QuantMaxPool2d, QuantDropout,
@@ -8,7 +8,7 @@ Public surface (mirrors the reference's module API for the quantized forward pat
   bit_config   bit_config_dict(), get_bit_config(arch, scheme), stamp_bit_config(model, cfg)
   engine       compile_model(model, example) -> CompiledModel (one CUDA graph per GPU), all_gather_logits
   ops / _lib   the C ABI (include/hawq_b200.h) through ctypes
-The frozen path runs only on the in-tree CUDA library (sm_100a); there is no CPU or PyTorch fallback.
+The frozen path runs only on the in-tree CUDA library (sm_90a); there is no CPU or PyTorch fallback.
 """
 from .modules import (QuantAct, QuantAveragePool2d, QuantBnConv2d, QuantConv2d, QuantDropout, QuantLinear,  # noqa: F401
                       QuantMaxPool2d, freeze_model, unfreeze_model)

@@ -1,6 +1,6 @@
 """ctypes binding of libhawq_b200.so (C ABI: include/hawq_b200.h).
 
-The library is built in-tree by ``hawq_b200.build.build_library`` (nvcc, sm_100a).  There is NO fallback: if the
+The library is built in-tree by ``hawq_b200.build.build_library`` (nvcc, sm_90a).  There is NO fallback: if the
 shared object is missing or cannot be loaded, every product entry point raises ``HawqLibraryError``.
 """
 import ctypes as C
@@ -81,8 +81,6 @@ SIGNATURES = {
     "hawq_permute_weights_for_i4": (_i32, [_vp, _i64, _i32]),
     "hawq_retile_weights": (_i32, [_vp, _vp, _i32, _i64, _vp, _vp]),
     "hawq_debug_kernel_count": (_i64, [_i32]),
-    "hawq_debug_halo_trace": (_i32, [_vp, _i32]),
-    "hawq_debug_c1_trace": (_i32, [_vp, _i32]),
     "hawq_workspace_bytes": (_i64, [C.POINTER(hawq_conv_desc), C.POINTER(hawq_epilogue_desc)]),
 }
 
@@ -97,7 +95,7 @@ def load():
     if not os.path.isfile(LIB_PATH):
         raise HawqLibraryError(
             "%s not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). hawq_b200 has no CPU or PyTorch fallback." % LIB_PATH)
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). hawq_b200 has no CPU or PyTorch fallback." % LIB_PATH)
     try:
         lib = C.CDLL(LIB_PATH)
     except OSError as e:

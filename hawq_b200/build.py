@@ -1,4 +1,4 @@
-"""In-tree build of libhawq_b200.so with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""In-tree build of libhawq_b200.so with nvcc for sm_90a (Hopper; cross-compiles without a GPU)."""
 import glob
 import os
 import shutil
@@ -9,7 +9,8 @@ CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 OUT = os.path.join(_HERE, "libhawq_b200.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 OBJ_DIR = os.path.join(_HERE, "_obj")
 
 
@@ -106,7 +107,7 @@ def build_library(force=False, verbose=False, extra_flags=()):
                 return OUT
             objs = _compile_objects(force, verbose, tuple(extra_flags))
             tmp = "%s.tmp.%d" % (OUT, os.getpid())
-            cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "--shared", "-o", tmp] + objs
+            cmd = [_nvcc()] + GENCODE + ["--shared", "-o", tmp] + objs
             if verbose:
                 print(" ".join(cmd).replace(tmp, OUT))
             r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)

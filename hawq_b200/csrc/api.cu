@@ -7,14 +7,9 @@
 
 #include <cstdlib>
 
-#include "conv1x1.h"
-#include "conv_dual.h"
-#include "conv_halo.h"
 #include "conv_igemm.cuh"
-#include "conv_tc.cuh"
 #include "elementwise.cuh"
 #include "stem.cuh"
-#include "stem_tc.h"
 
 using namespace hawq;
 
@@ -26,34 +21,6 @@ struct hawq_handle {
 
 static thread_local char g_err[512] = "";
 static long long g_kernel_count[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // hawq_debug_kernel_count: launches by kernel family (not atomic: debugging aid)
-
-// ---- TMA tensor maps (driver entry point resolved through the runtime: no link-time dependency on libcuda)
-typedef CUresult (*encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static encode_tiled_fn get_encode_tiled() {
-  static encode_tiled_fn fn = [] {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      ptr = nullptr;
-    return reinterpret_cast<encode_tiled_fn>(ptr);
-  }();
-  return fn;
-}
-// byte matrix [rows][inner_bytes] with row pitch pitch_bytes; box = box_inner bytes x box_rows rows
-static int make_map_2d(CUtensorMap* m, const void* base, uint64_t inner_bytes, uint64_t rows, uint64_t pitch_bytes, uint32_t box_inner,
-                       uint32_t box_rows, CUtensorMapSwizzle sw) {
-  encode_tiled_fn enc = get_encode_tiled();
-  if (!enc) return -1;
-  const cuuint64_t dims[2] = {inner_bytes, rows};
-  const cuuint64_t strides[1] = {pitch_bytes};
-  const cuuint32_t box[2] = {box_inner, box_rows};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : -1;
-}
 
 static int fail(int code, const char* fmt, ...) {
   va_list ap;
@@ -83,78 +50,31 @@ static int grid_for(long long work_items, int sm_count) {
   return (int)blocks;
 }
 
-template <int BN, bool A4, int EPI>
+template <int BN, bool A4, int EPI, bool DUAL>
 static int set_conv_attr1() {
-  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                ConvSmem<BN, A4>::TOTAL));
+  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, EPI, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                ConvSmem<BN, A4, DUAL>::TOTAL));
   return HAWQ_OK;
 }
 template <int BN, bool A4>
 static int set_conv_attr() {
   int rc;
-  if ((rc = set_conv_attr1<BN, A4, EPI_GENERIC>()) || (rc = set_conv_attr1<BN, A4, EPI_FAST_LOW>()) ||
-      (rc = set_conv_attr1<BN, A4, EPI_FAST_RES>()))
+  if ((rc = set_conv_attr1<BN, A4, EPI_GENERIC, false>()) || (rc = set_conv_attr1<BN, A4, EPI_FAST_LOW, false>()) ||
+      (rc = set_conv_attr1<BN, A4, EPI_FAST_RES, false>()) || (rc = set_conv_attr1<BN, A4, EPI_FAST_RES, true>()))
     return rc;
   return HAWQ_OK;
 }
 
-template <int EPI, bool WIDE>
-static int set_tc_attr1() {
-  CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<128, EPI, WIDE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<128, EPI, false>::TOTAL));
-  CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<64, EPI, WIDE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<64, EPI, false>::TOTAL));
-  CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<128, EPI, WIDE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<128, EPI, true>::TOTAL));
-  CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<64, EPI, WIDE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<64, EPI, true>::TOTAL));
-  return HAWQ_OK;
-}
-template <int EPI>
-static int set_tc_attr() {
-  int rc = set_tc_attr1<EPI, false>();
-  if (rc == HAWQ_OK && EPI >= TC_EPI_RES22) rc = set_tc_attr1<EPI, true>();
-  return rc;
-}
-
-// conv_tc launches carry the programmatic-stream-serialization attribute (HAWQ_B200_PDL != 0): the kernel's prologue may
-// start while the previous kernel of the stream drains; the kernel itself waits (griddepcontrol.wait) before touching memory
-template <int BN, int EPI, bool WIDE, bool A4>
-static void launch_tc3(const ConvParams& p, const TcMaps& maps, int grid, cudaStream_t st) {
-  static const bool pdl = [] { const char* e = getenv("HAWQ_B200_PDL"); return !(e && e[0] == '0'); }();
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)grid, 1, 1);
-  cfg.blockDim = dim3(TC_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = TcSmem<BN, EPI, A4>::TOTAL;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, EPI, WIDE, A4>, p, maps);   // errors surface through launch_check()
-}
-template <int EPI, bool WIDE, bool A4>
-static void launch_tc2(const ConvParams& p, const TcMaps& maps, bool bn128, int grid, cudaStream_t st) {
-  if (bn128) launch_tc3<128, EPI, WIDE, A4>(p, maps, grid, st);
-  else launch_tc3<64, EPI, WIDE, A4>(p, maps, grid, st);
-}
-template <int EPI>
-static void launch_tc(const ConvParams& p, const TcMaps& maps, bool bn128, bool ratios_wide, bool a4, int grid, cudaStream_t st) {
-  if constexpr (EPI >= TC_EPI_RES22) {
-    if (ratios_wide) {
-      if (a4) launch_tc2<EPI, true, true>(p, maps, bn128, grid, st);
-      else launch_tc2<EPI, true, false>(p, maps, bn128, grid, st);
-      return;
-    }
-  }
-  if (a4) launch_tc2<EPI, false, true>(p, maps, bn128, grid, st);
-  else launch_tc2<EPI, false, false>(p, maps, bn128, grid, st);
-}
-
 template <int BN, bool A4>
 static void launch_conv(const ConvParams& p, dim3 grid, cudaStream_t s) {
-  const int smem = ConvSmem<BN, A4>::TOTAL;
-  if (p.mode == HAWQ_EPI_REQUANT && p.out_bits <= 8) conv_igemm_kernel<BN, A4, EPI_FAST_LOW><<<grid, CONV_THREADS, smem, s>>>(p);
-  else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, EPI_FAST_RES><<<grid, CONV_THREADS, smem, s>>>(p);
-  else conv_igemm_kernel<BN, A4, EPI_GENERIC><<<grid, CONV_THREADS, smem, s>>>(p);
+  const int smem = ConvSmem<BN, A4, false>::TOTAL;
+  if (p.mode == HAWQ_EPI_REQUANT && p.out_bits <= 8) conv_igemm_kernel<BN, A4, EPI_FAST_LOW, false><<<grid, CONV_THREADS, smem, s>>>(p);
+  else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, EPI_FAST_RES, false><<<grid, CONV_THREADS, smem, s>>>(p);
+  else conv_igemm_kernel<BN, A4, EPI_GENERIC, false><<<grid, CONV_THREADS, smem, s>>>(p);
+}
+template <int BN, bool A4>
+static void launch_conv_dual(const ConvParams& p, dim3 grid, cudaStream_t s) {
+  conv_igemm_kernel<BN, A4, EPI_FAST_RES, true><<<grid, CONV_THREADS, ConvSmem<BN, A4, true>::TOTAL, s>>>(p);
 }
 
 extern "C" {
@@ -167,7 +87,8 @@ int hawq_create(int device, hawq_handle** out) {
   CUDA_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_create: device sm_%d%d is not Blackwell sm_100", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_create: device sm_%d%d is not Hopper sm_90 (the library is built for sm_90a)", prop.major, prop.minor);
   hawq_handle* h = new hawq_handle();
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
@@ -175,13 +96,6 @@ int hawq_create(int device, hawq_handle** out) {
   CUDA_TRY(cudaMalloc(&h->status, sizeof(int32_t)));
   CUDA_TRY(cudaMemset(h->status, 0, sizeof(int32_t)));
   int rc;
-  if ((rc = set_tc_attr<TC_EPI_REQ>()) || (rc = set_tc_attr<TC_EPI_RAW>()) || (rc = set_tc_attr<TC_EPI_RES22>()) ||
-      (rc = set_tc_attr<TC_EPI_RES44>()) || (rc = set_tc_attr<TC_EPI_RES42>()) || (rc = set_tc_attr<TC_EPI_DUAL>()))
-    return rc;
-  if ((rc = halo_set_attributes())) return fail(rc, "%s", halo_last_error());
-  if ((rc = c1_set_attributes())) return fail(rc, "%s", c1_last_error());
-  if ((rc = dual_set_attributes())) return fail(rc, "%s", dual_last_error());
-  if ((rc = stem_tc_set_attributes())) return fail(rc, "%s", stem_tc_last_error());
   CUDA_TRY(cudaFuncSetAttribute(linear_dp4a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, linear_smem_bytes(LIN_MAX_K)));
   if ((rc = set_conv_attr<128, false>()) || (rc = set_conv_attr<64, false>()) || (rc = set_conv_attr<128, true>()) ||
       (rc = set_conv_attr<64, true>()))
@@ -218,14 +132,6 @@ int hawq_copy_status(hawq_handle* h, int32_t* dst, void* stream) {
   return HAWQ_OK;
 }
 
-static bool sat_pack_enabled() {
-  static const bool on = [] { const char* e = getenv("HAWQ_B200_SATPACK"); return !(e && e[0] == '0'); }();
-  return on;
-}
-
-// scalar dyadic pairs whose folded FMA constant (magic - 2^52 * m * 2^-e) is exact in the tcgen05 RESIDUAL epilogues
-static bool fold_ok(uint32_t m, int e) { return m == 0u || e <= 51; }
-
 static int check_me(uint32_t m, int e, const char* what) {
   if (e < 1 || e > 62 || m > 0x80000000u) return fail(HAWQ_ERR_BAD_ARG, "%s: dyadic pair out of range (m=%u e=%d)", what, m, e);
   return HAWQ_OK;
@@ -259,14 +165,11 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
   p.y_bits = ep->y_bits; p.low_bits = ep->low_bits; p.low_m = ep->low_m; p.low_e = ep->low_e;
   p.low_lo = ep->low_lo; p.low_hi = ep->low_hi; p.cout_store = ep->cout_store;
   p.slow_scalar = 0;
-  p.tma_a = 0;
-  p.tma_io = 0;
-  p.patch_rows = 0;
-  p.w_tiled = nullptr;
-  p.sat_pack = sat_pack_enabled() ? 1 : 0;
+  p.check_ovf = ep->mode == HAWQ_EPI_RESIDUAL && (ep->flags & (HAWQ_EP_RATIOS_LE_ONE | HAWQ_EP_RATIOS_LE_2P20)) != 0;
   if (ep->mode == HAWQ_EPI_RESIDUAL) {
     if (ep->res_kind == 0 && !dyadic_is_fast(ep->res_m, ep->res_e)) p.slow_scalar = 1;
     if (ep->low_bits != 0 && !dyadic_is_fast(ep->low_m, ep->low_e)) p.slow_scalar = 1;
+    p.wide_scalar_bad = (ep->res_kind == 0 && !dyadic_is_wide(ep->res_m, ep->res_e)) || (ep->low_bits != 0 && !dyadic_is_fast(ep->low_m, ep->low_e));
   }
 
   switch (ep->mode) {
@@ -307,76 +210,7 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
       return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: unknown epilogue mode %d", ep->mode);
   }
 
-  // tcgen05 path: int8 activations, the three hot epilogues, all ratios <= 1 (promised), HAWQ_B200_TC != 0
-  static const bool tc_enabled = [] { const char* e = getenv("HAWQ_B200_TC"); return !(e && e[0] == '0'); }();
-  const bool tc_epi = (ep->mode == HAWQ_EPI_REQUANT && ep->out_bits <= 8) || (ep->mode == HAWQ_EPI_RESIDUAL && ep->y_bits != 0 && ep->relu) ||
-                      ep->mode == HAWQ_EPI_RAW_I32;
-  const bool ratios_one = (ep->flags & HAWQ_EP_RATIOS_LE_ONE) != 0;
-  const bool ratios_wide = !ratios_one && (ep->flags & HAWQ_EP_RATIOS_LE_2P20) != 0 && ep->mode == HAWQ_EPI_RESIDUAL;
-  const bool folds = ep->mode != HAWQ_EPI_RESIDUAL || ((ep->res_kind != 0 || fold_ok(ep->res_m, ep->res_e)) && (ep->low_bits == 0 || fold_ok(ep->low_m, ep->low_e)));
-  if (tc_enabled && tc_epi && folds && (ratios_one || ratios_wide)) {
-    const bool a4 = d->a_bits == 4;
-    // 3x3 stride-1 REQUANT layers: A operand read in place from a zero-padded TMA patch, weights stationary (conv_halo.cuh)
-    if (ep->mode == HAWQ_EPI_REQUANT) {
-      const int hr = launch_conv_halo(h->sm_count, d, ep, x, w, chan, out, h->status, stream);
-      if (hr < 0) return fail(hr, "%s", halo_last_error());
-      if (hr == 0 || hr == 2) { ++g_kernel_count[1]; g_kernel_count[2] += hr == 2; return launch_check("conv_halo"); }
-    }
-    // 1x1 stride-1 layers (REQUANT, uint16-stream RESIDUAL): stationary weights, large TMA copies (conv1x1.cuh)
-    if (ep->mode == HAWQ_EPI_REQUANT || ep->mode == HAWQ_EPI_RESIDUAL) {
-      const int cr = launch_conv1x1(h->sm_count, d, ep, x, w, chan, res, out, out_low, h->status, p.sat_pack, stream);
-      if (cr < 0) return fail(cr, "%s", c1_last_error());
-      if (cr == 0) { ++g_kernel_count[3]; return launch_check("conv1x1"); }
-    }
-    ++g_kernel_count[0];
-    const int bn = (d->Cout % 128 == 0) ? 128 : 64;
-    TcMaps maps;
-    memset(&maps, 0, sizeof(maps));
-    if (d->w_layout == 1) p.w_tiled = w + (size_t)d->Cout * p.K;     // caller appended the re-tiled copy (hawq_retile_weights)
-    else if (make_map_2d(&maps.b, w, (uint64_t)p.K, (uint64_t)d->Cout, (uint64_t)p.K, 64, (uint32_t)bn, CU_TENSOR_MAP_SWIZZLE_64B))
-      return fail(HAWQ_ERR_CUDA, "hawq_conv2d: cuTensorMapEncodeTiled (weights) failed");
-    p.tma_a = (!a4 && d->kh == 1 && d->kw == 1 && d->stride == 1 && d->pad == 0) ? 1 : 0;
-    if (p.tma_a && make_map_2d(&maps.a, x, (uint64_t)d->Cin, (uint64_t)M, (uint64_t)d->Cin, 64, TC_BM, CU_TENSOR_MAP_SWIZZLE_64B))
-      return fail(HAWQ_ERR_CUDA, "hawq_conv2d: cuTensorMapEncodeTiled (activations) failed");
-    const bool wide = (d->Cout % 128 == 0);
-    const long long tiles = ((M + TC_BM - 1) / TC_BM) * (d->Cout / (wide ? 128 : 64));
-    const int grid = (int)(tiles < h->sm_count ? tiles : h->sm_count);
-    cudaStream_t st = (cudaStream_t)stream;
-    static const bool patch_enabled = [] { const char* e = getenv("HAWQ_B200_PATCH"); return !(e && e[0] == '0'); }();
-    if (patch_enabled && ep->mode == HAWQ_EPI_REQUANT && d->kh == 3 && d->kw == 3 && d->stride == 1 && d->pad == 1 && 128 + 2 * d->W + 2 <= 256) {
-      const uint32_t rows = 128 + 2 * d->W + 2;
-      const uint32_t rowb = a4 ? 32 : 64;
-      if (make_map_2d(&maps.patch, x, (uint64_t)p.x_pix_bytes, (uint64_t)d->N * d->H * d->W, (uint64_t)p.x_pix_bytes, rowb, rows,
-                      a4 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B))
-        return fail(HAWQ_ERR_CUDA, "hawq_conv2d: cuTensorMapEncodeTiled (input patch) failed");
-      p.patch_rows = (int)rows;
-    }
-    if (ep->mode == HAWQ_EPI_RESIDUAL && ep->res_kind == 0 && ep->res_bits == 16 && ep->y_bits == 16) {
-      const uint32_t cw = bn / 2;   // columns per epilogue warp
-      const CUtensorMapSwizzle sw_y = cw * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-      int bad = make_map_2d(&maps.res, res, (uint64_t)d->Cout * 2, (uint64_t)M, (uint64_t)d->Cout * 2, cw * 2, 32, sw_y);
-      bad |= make_map_2d(&maps.y, out, (uint64_t)d->Cout * 2, (uint64_t)M, (uint64_t)d->Cout * 2, cw * 2, 32, sw_y);
-      if (ep->low_bits) {
-        const uint32_t lb = cw * ep->low_bits / 8;   // low tile row bytes: 64 / 32 / 16
-        const CUtensorMapSwizzle sw_l = lb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : lb == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
-        bad |= make_map_2d(&maps.low, out_low, (uint64_t)d->Cout * ep->low_bits / 8, (uint64_t)M, (uint64_t)d->Cout * ep->low_bits / 8, lb, 32, sw_l);
-      }
-      if (bad) return fail(HAWQ_ERR_CUDA, "hawq_conv2d: cuTensorMapEncodeTiled (residual epilogue) failed");
-      p.tma_io = 1;
-    }
-    if (ep->mode == HAWQ_EPI_REQUANT) launch_tc<TC_EPI_REQ>(p, maps, wide, false, a4, grid, st);
-    else if (ep->mode == HAWQ_EPI_RAW_I32) launch_tc<TC_EPI_RAW>(p, maps, wide, false, a4, grid, st);
-    else {
-      const int res_es = (ep->res_kind == 1 || ep->res_bits == 32) ? 4 : 2;
-      if (res_es == 2 && ep->y_bits == 16) launch_tc<TC_EPI_RES22>(p, maps, wide, ratios_wide, a4, grid, st);
-      else if (res_es == 4 && ep->y_bits == 32) launch_tc<TC_EPI_RES44>(p, maps, wide, ratios_wide, a4, grid, st);
-      else if (res_es == 4 && ep->y_bits == 16) launch_tc<TC_EPI_RES42>(p, maps, wide, ratios_wide, a4, grid, st);
-      else goto legacy;   // uint16 residual in, int32 out: not a combination the engine produces
-    }
-    return launch_check("conv_tc");
-  }
-
-legacy:
+  ++g_kernel_count[0];
   const bool bn128 = (d->Cout % 128 == 0);
   const dim3 grid((unsigned)((M + CONV_BM - 1) / CONV_BM), (unsigned)(d->Cout / (bn128 ? 128 : 64)), 1);
   cudaStream_t s = (cudaStream_t)stream;
@@ -391,14 +225,11 @@ legacy:
 }
 
 // Resize-unit fusion: y = RHE(m1 * (conv1x1_s(x2, w2) + bias2)) + RHE(m * (conv1x1(x, w) + bias)), ReLU, uint16 stream +
-// optional low-bit copy.  Both convolutions accumulate in TMEM inside one kernel (no int32 identity tensor in HBM).
+// optional low-bit copy.  Both convolutions run in one kernel; the identity result stays in shared memory (no int32 tensor in HBM).
 int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_desc* ep, const void* x, const int8_t* w,
                      const hawq_chan* chan, const hawq_conv_desc* d2, const void* x2, const int8_t* w2, const hawq_chan* chan2,
                      void* out, void* out_low, void* stream) {
   if (!h || !d || !ep || !x || !w || !chan || !d2 || !x2 || !w2 || !chan2 || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: null argument");
-  static const bool tc_enabled = [] { const char* e = getenv("HAWQ_B200_TC"); return !(e && e[0] == '0'); }();
-  static const bool dual_enabled = [] { const char* e = getenv("HAWQ_B200_DUAL"); return !(e && e[0] == '0'); }();
-  if (!tc_enabled || !dual_enabled) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: disabled by environment");
   if (d->kh != 1 || d->kw != 1 || d->stride != 1 || d->pad != 0 || d2->kh != 1 || d2->kw != 1 || d2->pad != 0 || d2->stride < 1)
     return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: both convolutions must be 1x1 without padding (main stride 1)");
   if (d->N < 1 || d->H < 1 || d->W < 1 || d2->H < 1 || d2->W < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: bad geometry");
@@ -413,7 +244,7 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
     if (!out_low) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: low_bits set but out_low is null");
     int rc = check_me(ep->low_m, ep->low_e, "hawq_conv2d_dual low-bit copy");
     if (rc) return rc;
-    if (!dyadic_is_fast(ep->low_m, ep->low_e) || !fold_ok(ep->low_m, ep->low_e)) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: low-bit ratio outside the fast range");
+    if (!dyadic_is_fast(ep->low_m, ep->low_e)) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: low-bit ratio outside the fast range");
   }
   const bool ratios_one = (ep->flags & HAWQ_EP_RATIOS_LE_ONE) != 0;
   const bool ratios_wide = !ratios_one && (ep->flags & HAWQ_EP_RATIOS_LE_2P20) != 0;
@@ -421,43 +252,29 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
   const long long M = (long long)d->N * d->H * d->W;
   if (M > 0x7fffff00ll || (long long)d2->N * d2->H * d2->W > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: too many pixels");
 
-  {   // int8 resize units: stationary weights, strided identity rows by TMA (conv_dual.cuh)
-    const int dr = launch_conv_dual(h->sm_count, d, ep, x, w, chan, d2, x2, w2, chan2, out, out_low, h->status, sat_pack_enabled() ? 1 : 0, stream);
-    if (dr < 0) return fail(dr, "%s", dual_last_error());
-    if (dr == 0) { ++g_kernel_count[4]; return launch_check("conv_dual"); }
-  }
-  ++g_kernel_count[5];
+  ++g_kernel_count[4];
   ConvParams p;
   memset(&p, 0, sizeof(p));
-  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = out; p.out_low = out_low; p.status = h->status;
+  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.res_chan = chan2; p.out = out; p.out_low = out_low; p.status = h->status;
   p.N = d->N; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout; p.KH = 1; p.KW = 1; p.stride = 1; p.pad = 0;
   p.Ho = d->H; p.Wo = d->W; p.M = (int)M; p.K = d->Cin; p.cin_chunks = d->Cin / 64; p.x_pix_bytes = d->Cin * d->a_bits / 8;
-  p.mode = ep->mode; p.relu = 1; p.res_kind = 1; p.y_bits = 16; p.low_bits = ep->low_bits; p.low_m = ep->low_m; p.low_e = ep->low_e;
-  p.low_lo = ep->low_lo; p.low_hi = ep->low_hi;
-  p.w_tiled = w + (size_t)d->Cout * d->Cin;
-  p.dual = 1;
-  p.sat_pack = sat_pack_enabled() ? 1 : 0;
-  p.x2 = (const uint8_t*)x2; p.w2_tiled = w2 + (size_t)d2->Cout * d2->Cin; p.chan2 = chan2;
-  p.H2 = d2->H; p.W2 = d2->W; p.stride2 = d2->stride; p.cin_chunks2 = d2->Cin / 64; p.x2_pix_bytes = d2->Cin * d2->a_bits / 8;
-  p.tma_io = 1;
+  p.mode = HAWQ_EPI_RESIDUAL; p.relu = 1; p.res_kind = 1; p.res_bits = 32; p.y_bits = 16; p.low_bits = ep->low_bits; p.low_m = ep->low_m;
+  p.low_e = ep->low_e; p.low_lo = ep->low_lo; p.low_hi = ep->low_hi;
+  p.check_ovf = 1;
+  p.x2 = (const uint8_t*)x2; p.w2 = w2; p.H2 = d2->H; p.W2 = d2->W; p.stride2 = d2->stride; p.cin_chunks2 = d2->Cin / 64;
+  p.x2_pix_bytes = d2->Cin * d2->a_bits / 8;
 
-  const bool a4 = d->a_bits == 4;
   const bool bn128 = (d->Cout % 128 == 0);
-  const uint32_t cw = (bn128 ? 128 : 64) / 2;
-  TcMaps maps;
-  memset(&maps, 0, sizeof(maps));
-  const CUtensorMapSwizzle sw_y = cw * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  int bad = make_map_2d(&maps.y, out, (uint64_t)d->Cout * 2, (uint64_t)M, (uint64_t)d->Cout * 2, cw * 2, 32, sw_y);
-  if (ep->low_bits) {
-    const uint32_t lb = cw * ep->low_bits / 8;
-    const CUtensorMapSwizzle sw_l = lb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : lb == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
-    bad |= make_map_2d(&maps.low, out_low, (uint64_t)d->Cout * ep->low_bits / 8, (uint64_t)M, (uint64_t)d->Cout * ep->low_bits / 8, lb, 32, sw_l);
+  const dim3 grid((unsigned)((M + CONV_BM - 1) / CONV_BM), (unsigned)(d->Cout / (bn128 ? 128 : 64)), 1);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (d->a_bits == 8) {
+    if (bn128) launch_conv_dual<128, false>(p, grid, s);
+    else launch_conv_dual<64, false>(p, grid, s);
+  } else {
+    if (bn128) launch_conv_dual<128, true>(p, grid, s);
+    else launch_conv_dual<64, true>(p, grid, s);
   }
-  if (bad) return fail(HAWQ_ERR_CUDA, "hawq_conv2d_dual: cuTensorMapEncodeTiled failed");
-  const long long tiles = ((M + TC_BM - 1) / TC_BM) * (d->Cout / (bn128 ? 128 : 64));
-  const int grid = (int)(tiles < h->sm_count ? tiles : h->sm_count);
-  launch_tc<TC_EPI_DUAL>(p, maps, bn128, ratios_wide, a4, grid, (cudaStream_t)stream);
-  return launch_check("conv_tc_dual");
+  return launch_check("conv_dual");
 }
 
 int hawq_conv2d_i8(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_desc* ep, const void* x,
@@ -518,12 +335,17 @@ int hawq_stem_pool_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int
   if ((y_bits != 16 && y_bits != 32) || (low_bits != 0 && low_bits != 4 && low_bits != 8) || (low_bits && !out_low))
     return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_pool_i8: bad output description");
   if (low_bits) { int rc = check_me(low_m, low_e, "hawq_stem_pool_i8"); if (rc) return rc; }
-  const int r = launch_stem_tc(h->sm_count, N, H, W, x, w256, chan, clamp_lo, clamp_hi, y_bits, y, low_bits, low_m, low_e, low_lo, low_hi, out_low,
-                               h->status, stream);
-  if (r < 0) return fail(r, "%s", stem_tc_last_error());
-  if (r == 1) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_pool_i8: shape / ratio outside the fused kernel (use hawq_stem_conv_i8 + hawq_maxpool_requant)");
+  if (W % 16 != 0 || W > 256 || (low_bits && !dyadic_is_fast(low_m, low_e)))
+    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_pool_i8: shape / ratio outside the fused kernel (use hawq_stem_conv_i8 + hawq_maxpool_requant)");
+  if (N > 65535) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_pool_i8: N > 65535");
+  const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
+  const int Po = (Ho + 2 - 3) / 2 + 1, Qo = (Wo + 2 - 3) / 2 + 1;
+  const long long tiles = (long long)N * ((Po + STEMP_PH - 1) / STEMP_PH) * ((Qo + STEMP_PW - 1) / STEMP_PW);
+  const int ctas = (int)(tiles < 4LL * h->sm_count ? tiles : 4LL * h->sm_count);
   ++g_kernel_count[6];
-  return launch_check("stem_tc");
+  stem_pool_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(x, (const uint32_t*)w256, chan, N, H, W, Ho, Wo, Po, Qo, clamp_lo, clamp_hi, y_bits, y,
+                                                          low_bits, low_m, low_e, low_lo, low_hi, out_low);
+  return launch_check("stem_pool");
 }
 
 int hawq_maxpool_requant(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_t C, const int16_t* x, int32_t y_bits,
@@ -672,8 +494,6 @@ int hawq_retile_weights(hawq_handle* h, const int8_t* w_ohwi, int32_t Cout, int6
   return launch_check("retile_weights");
 }
 
-int32_t hawq_debug_halo_trace(int64_t* host_out, int32_t n) { return halo_read_trace(reinterpret_cast<long long*>(host_out), n); }
-int32_t hawq_debug_c1_trace(int64_t* host_out, int32_t n) { return c1_read_trace(reinterpret_cast<long long*>(host_out), n); }
 
 int64_t hawq_debug_kernel_count(int32_t family) { return (family >= 0 && family < 8) ? g_kernel_count[family] : -1; }
 

@@ -12,16 +12,20 @@ namespace hawq {
 // identical while |v*m| < 2^53 (the reference's own exactness envelope, SURVEY.md A.6), exact beyond it.
 // Preconditions: m <= 2^31, 1 <= e <= 62.  Result saturated to int32.
 // ---------------------------------------------------------------------------------------------------------
-__host__ __device__ __forceinline__ int32_t rhe_requant(int32_t v, uint32_t m, int32_t e) {
+__host__ __device__ __forceinline__ long long rhe_requant64(int32_t v, uint32_t m, int32_t e) {   // unsaturated
   const long long p = (long long)v * (long long)(unsigned long long)m;  // |p| <= 2^62
   long long q = p >> e;                                                  // floor
   const unsigned long long rem = (unsigned long long)p & ((1ull << e) - 1ull);
   const unsigned long long half = 1ull << (e - 1);
   q += (long long)((rem > half) | ((rem == half) & (unsigned long long)(q & 1)));
+  return q;
+}
+__host__ __device__ __forceinline__ int32_t sat_i32(long long q) {
   q = q > 2147483647ll ? 2147483647ll : q;
   q = q < -2147483648ll ? -2147483648ll : q;
   return (int32_t)q;
 }
+__host__ __device__ __forceinline__ int32_t rhe_requant(int32_t v, uint32_t m, int32_t e) { return sat_i32(rhe_requant64(v, m, e)); }
 
 __device__ __forceinline__ int32_t clampi(int32_t v, int32_t lo, int32_t hi) { return max(lo, min(v, hi)); }
 
@@ -44,6 +48,8 @@ __device__ __forceinline__ double dyadic_to_double(uint32_t m, int32_t e) {
   return (double)m * __hiloint2double((1023 - e) << 20, 0);   // m * 2^-e, exact
 }
 __host__ __device__ __forceinline__ bool dyadic_is_fast(uint32_t m, int32_t e) { return m == 0u || e >= 31; }
+// ratio m * 2^-e <= 2^20: |v| < 2^32 times M stays below 2^52, so the one-FMA form is exact whenever its result fits int32
+__host__ __device__ __forceinline__ bool dyadic_is_wide(uint32_t m, int32_t e) { return m == 0u || e >= 11; }
 
 __device__ __forceinline__ int32_t rhe_requant_fast(int32_t v, double M) {
   const double dv = __hiloint2double(0x43300000, (int)((uint32_t)v ^ 0x80000000u)) - 4503601774854144.0;

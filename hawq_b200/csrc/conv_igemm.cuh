@@ -1,13 +1,17 @@
-// Implicit-GEMM integer convolution with fused HAWQ epilogues (stage-A kernel: IMMA m16n8k32 + cp.async pipeline).
+// Implicit-GEMM integer convolution with fused HAWQ epilogues (Hopper: warpgroup MMA + cp.async pipeline).
 //
 //   M = N*Ho*Wo output pixels, N = Cout, K = kh*kw*Cin.   A[m,k] gathered on the fly from the NHWC activation
-//   tensor (zero-filled outside the image), B = int8 OHWI weights.  CTA tile 128 x BN x 64 channels, 8 warps
-//   (4 along M x 2 along N), 4-stage cp.async ring, XOR-swizzled shared memory read with ldmatrix.
+//   tensor (zero-filled outside the image), B = int8 OHWI weights.  CTA tile 128 x BN x 64 channels, 2 warpgroups of
+//   64 output rows each issuing wgmma m64nBNk32 (wgmma.cuh), 4-stage cp.async ring, shared-memory tiles in the
+//   SWIZZLE_64B layout the wgmma descriptors read.
 //
 //   A4 = true: activations are packed unsigned nibbles (hawq nibble order).  They stay packed in HBM and in shared
 //   memory (half the bytes); each ldmatrix word (8 nibbles) is expanded in registers with AND / SHIFT+AND into the
-//   two int8x4 words of the MMA A fragment.  The weight rows of such layers are K-permuted on the host so that the
+//   two int8x4 words of the register A fragment.  The weight rows of such layers are K-permuted on the host so that the
 //   expansion needs no shuffles (hawq_permute_weights_for_i4).
+//
+//   DUAL = true (resize units): the identity-branch 1x1 convolution (x2, w2) runs first in the same CTA; its int32 result
+//   (acc + bias2) stays in shared memory as the res_kind 1 operand of the RESIDUAL epilogue of the main convolution.
 //
 //   Epilogues (hawq_epilogue_mode): REQUANT (case 0 of fixedpoint_fn), RESIDUAL (case 1: dual dyadic requant + add,
 //   optional ReLU, writes the new residual stream and/or the next unit's low-bit activation), RAW_I32, DEQUANT_F32.
@@ -15,6 +19,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace hawq {
 
@@ -40,17 +45,11 @@ struct ConvParams {
   int low_e, low_lo, low_hi;
   int cout_store;
   int slow_scalar;   // host-checked: a scalar dyadic pair (res / low) has ratio > 1 -> generic 64-bit requant
-  int tma_a;         // tcgen05 kernel: activations are fetched by TMA (1x1 stride-1 int8 layers)
-  int tma_io;        // tcgen05 kernel: uint16 residual tile in / outputs out through TMA
-  const int8_t* w_tiled;  // tcgen05 kernel: weights re-tiled into contiguous pre-swizzled [n_tile][k_tile][BN][64] blocks
-  int patch_rows;    // tcgen05 kernel, 3x3 stride-1 pad-1 layers: rows of the shared-memory input patch (128 + 2W + 2), 0 = gather mode
-  int sat_pack;           // tcgen05 RESIDUAL epilogues: 8-bit low copy packed with cvt.pack.sat when its clamp is [<= 0, 127]
-  // tcgen05 dual mode (resize units): the identity-branch 1x1 convolution is computed in the same kernel into a second
-  // TMEM accumulator instead of round-tripping an int32 tensor through HBM
-  int dual;               // 0 / 1
-  const uint8_t* x2;      // identity conv input (same a_bits as x)
-  const int8_t* w2_tiled; // its re-tiled weights
-  const hawq_chan* chan2; // its bias and the case-1 identity ratio (m1, e1) per channel
+  int wide_scalar_bad;   // host-checked: the scalar residual ratio exceeds 2^20 or the low-bit ratio exceeds 1 (no WIDE epilogue)
+  int check_ovf;     // RESIDUAL under a HAWQ_EP_RATIOS_* promise: a requantised term leaving int32 raises HAWQ_FLAG_REQUANT_OVERFLOW
+  // DUAL launches: the identity 1x1 convolution (res_chan holds its bias and per-channel identity ratio)
+  const uint8_t* x2;
+  const int8_t* w2;
   int H2, W2, stride2, cin_chunks2, x2_pix_bytes;
 };
 
@@ -58,7 +57,7 @@ constexpr int CONV_BM = 128;
 constexpr int CONV_STAGES = 4;
 constexpr int CONV_THREADS = 256;
 
-template <int BN, bool A4>
+template <int BN, bool A4, bool DUAL>
 struct ConvSmem {
   static constexpr int A_ROW = A4 ? 32 : 64;  // bytes of one A row per k-tile (64 channels)
   static constexpr int A_STAGE = CONV_BM * A_ROW;
@@ -67,7 +66,9 @@ struct ConvSmem {
   static constexpr int OUT_PITCH = BN + 16;
   static constexpr int OUT_STAGE = CONV_BM * OUT_PITCH;
   static constexpr int RES_TILE = CONV_BM * (BN * 4 + 32);                 // residual tile, worst case int32 + padding
-  static constexpr int MAIN = PIPE > RES_TILE ? PIPE : RES_TILE;          // pipeline ring, later the residual / y tile
+  // the residual / y tile reuses the pipeline ring, except in DUAL launches (filled before the main convolution's k loop)
+  static constexpr int RES_OFF = DUAL ? PIPE : 0;
+  static constexpr int MAIN = DUAL ? PIPE + RES_TILE : (PIPE > RES_TILE ? PIPE : RES_TILE);
   static constexpr int OUT_OFF = MAIN;                                     // low-bit output staging tile
   static constexpr int CHAN_OFF = OUT_OFF + OUT_STAGE;                     // hawq_chan[BN]
   static constexpr int M_OFF = CHAN_OFF + BN * (int)sizeof(hawq_chan);     // double[BN]: m * 2^-e of chan
@@ -88,19 +89,26 @@ __device__ __forceinline__ int swz(int row, int ch) {
 // kernel verifies): 0 = none (generic run-time epilogue only), 1 = REQUANT to 4/8 bits, 2 = RESIDUAL.
 constexpr int EPI_GENERIC = 0, EPI_FAST_LOW = 1, EPI_FAST_RES = 2;
 
-template <int BN, bool A4, int EPI>
+// geometry of one implicit GEMM of a launch (the main convolution, or the identity convolution of a DUAL launch)
+struct ConvGeom {
+  const uint8_t* x;
+  const int8_t* w;
+  int H, W, stride, pad, KH, KW, cin_chunks, x_pix_bytes, K;
+};
+
+template <int BN, bool A4, int EPI, bool DUAL>
 __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvParams p) {
-  using S = ConvSmem<BN, A4>;
+  using S = ConvSmem<BN, A4, DUAL>;
   constexpr int BM = CONV_BM, STAGES = CONV_STAGES;
   constexpr int A_ROW = S::A_ROW;
   constexpr int A_CH = A_ROW / 16;                    // 16-byte chunks per A row: 4 or 2
   constexpr int A_ROWS_PER_PASS = CONV_THREADS / A_CH;  // 64 or 128
   constexpr int A_PASSES = BM / A_ROWS_PER_PASS;        // 2 or 1
   constexpr int B_PASSES = BN / 64;
-  constexpr int WNT = BN / 2;   // warp tile width
-  constexpr int NT = WNT / 8;   // n8 tiles per warp: 8 or 4
+  constexpr int NT = BN / 8;    // 8-column blocks of the accumulator: 16 or 8
+  constexpr int NACC = BN / 2;  // accumulator registers per thread
 
-  extern __shared__ __align__(128) uint8_t smem[];
+  extern __shared__ __align__(1024) uint8_t smem[];   // 512-B aligned tiles: the wgmma descriptors address them swizzled
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * S::A_STAGE;
   hawq_chan* sChan = reinterpret_cast<hawq_chan*>(smem + S::CHAN_OFF);
@@ -111,135 +119,148 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
 
   const int tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5;
-  const int wm = warp & 3, wn = warp >> 2;
+  const int wg = warp >> 2;     // warpgroup: output rows 64 * wg ... 64 * wg + 63
   const int g = lane >> 2, t = lane & 3;
   const int m0 = blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
 
   int slow = p.slow_scalar;
+  int wide_bad = p.wide_scalar_bad;   // some ratio > 2^20: the FP64 FMA is no longer exact for every int32 operand
   if (tid < BN) {
     const hawq_chan c = p.chan[n0 + tid];
     sChan[tid] = c;
     sM[tid] = dyadic_to_double(c.m, c.e);
     sCb[tid] = 4503601774854144.0 - (double)c.bias;   // exact: folds the bias add into the int -> double conversion
     slow |= !dyadic_is_fast(c.m, c.e);
+    wide_bad |= !dyadic_is_wide(c.m, c.e);
     if (p.mode == HAWQ_EPI_RESIDUAL && p.res_kind == 1) {
       const hawq_chan rc = p.res_chan[n0 + tid];
       sResChan[tid] = rc;
       sM1[tid] = dyadic_to_double(rc.m, rc.e);
       slow |= !dyadic_is_fast(rc.m, rc.e);
+      wide_bad |= !dyadic_is_wide(rc.m, rc.e);
     }
   }
   const bool use_slow = __syncthreads_or(slow) != 0;   // CTA-uniform: any ratio > 1 -> generic exact integer requant
+  // RESIDUAL under a ratio promise with every ratio <= 2^20: the FP64 epilogue stays exact whenever a term fits int32, and every term
+  // is range-checked (HAWQ_FLAG_REQUANT_OVERFLOW), so it replaces the generic epilogue (CTA-uniform)
+  const bool use_wide = (__syncthreads_or(wide_bad) == 0) && use_slow && p.check_ovf && p.mode == HAWQ_EPI_RESIDUAL;
 
-  // ---- per-thread gather coordinates for the A rows this thread copies ----
-  const int a_ch = tid % A_CH;
-  int a_hi0[A_PASSES], a_wi0[A_PASSES], a_pix[A_PASSES];
-  bool a_ok[A_PASSES];
+  int32_t acc[NACC];
+
+  // acc = A(128 x K) * B(K x BN) of geometry gm for this CTA's tile
+  auto gemm = [&](const ConvGeom& gm) {
 #pragma unroll
-  for (int i = 0; i < A_PASSES; ++i) {
-    const int row = tid / A_CH + i * A_ROWS_PER_PASS;
-    const int m = m0 + row;
-    a_ok[i] = m < p.M;
-    const int mm = a_ok[i] ? m : 0;
-    const int n = mm / (p.Ho * p.Wo);
-    const int r = mm - n * (p.Ho * p.Wo);
-    const int ho = r / p.Wo, wo = r - ho * p.Wo;
-    a_hi0[i] = ho * p.stride - p.pad;
-    a_wi0[i] = wo * p.stride - p.pad;
-    a_pix[i] = n * p.H * p.W;
-  }
-  const int b_ch = tid & 3, b_row = tid >> 2;
-  const int KT = p.KH * p.KW * p.cin_chunks;
-  int ld_c = 0, ld_kw = 0, ld_kh = 0, ld_kt = 0;
-
-  auto load_tile = [&](int stage) {
-    const uint32_t a_base = smem_u32(sA + stage * S::A_STAGE);
+    for (int i = 0; i < NACC; ++i) acc[i] = 0;
+    // per-thread gather coordinates for the A rows this thread copies
+    const int a_ch = tid % A_CH;
+    int a_hi0[A_PASSES], a_wi0[A_PASSES], a_pix[A_PASSES];
+    bool a_ok[A_PASSES];
 #pragma unroll
     for (int i = 0; i < A_PASSES; ++i) {
       const int row = tid / A_CH + i * A_ROWS_PER_PASS;
-      const int hi = a_hi0[i] + ld_kh, wi = a_wi0[i] + ld_kw;
-      const bool v = a_ok[i] && (unsigned)hi < (unsigned)p.H && (unsigned)wi < (unsigned)p.W;
-      const uint8_t* src = p.x;
-      if (v) src = p.x + (size_t)(a_pix[i] + hi * p.W + wi) * p.x_pix_bytes + ld_c * A_ROW + a_ch * 16;
-      cp_async_16(a_base + swz<A_ROW>(row, a_ch), src, v ? 16 : 0);
+      const int m = m0 + row;
+      a_ok[i] = m < p.M;
+      const int mm = a_ok[i] ? m : 0;
+      const int n = mm / (p.Ho * p.Wo);
+      const int r = mm - n * (p.Ho * p.Wo);
+      const int ho = r / p.Wo, wo = r - ho * p.Wo;
+      a_hi0[i] = ho * gm.stride - gm.pad;
+      a_wi0[i] = wo * gm.stride - gm.pad;
+      a_pix[i] = n * gm.H * gm.W;
     }
-    const uint32_t b_base = smem_u32(sB + stage * S::B_STAGE);
+    const int b_ch = tid & 3, b_row = tid >> 2;
+    const int KT = gm.KH * gm.KW * gm.cin_chunks;
+    int ld_c = 0, ld_kw = 0, ld_kh = 0, ld_kt = 0;
+
+    auto load_tile = [&](int stage) {
+      const uint32_t a_base = smem_u32(sA + stage * S::A_STAGE);
 #pragma unroll
-    for (int i = 0; i < B_PASSES; ++i) {
-      const int row = b_row + i * 64;
-      const int8_t* src = p.w + (size_t)(n0 + row) * p.K + ld_kt * 64 + b_ch * 16;
-      cp_async_16(b_base + swz<64>(row, b_ch), src, 16);
+      for (int i = 0; i < A_PASSES; ++i) {
+        const int row = tid / A_CH + i * A_ROWS_PER_PASS;
+        const int hi = a_hi0[i] + ld_kh, wi = a_wi0[i] + ld_kw;
+        const bool v = a_ok[i] && (unsigned)hi < (unsigned)gm.H && (unsigned)wi < (unsigned)gm.W;
+        const uint8_t* src = gm.x;
+        if (v) src = gm.x + (size_t)(a_pix[i] + hi * gm.W + wi) * gm.x_pix_bytes + ld_c * A_ROW + a_ch * 16;
+        cp_async_16(a_base + swz<A_ROW>(row, a_ch), src, v ? 16 : 0);
+      }
+      const uint32_t b_base = smem_u32(sB + stage * S::B_STAGE);
+#pragma unroll
+      for (int i = 0; i < B_PASSES; ++i) {
+        const int row = b_row + i * 64;
+        const int8_t* src = gm.w + (size_t)(n0 + row) * gm.K + ld_kt * 64 + b_ch * 16;
+        cp_async_16(b_base + swz<64>(row, b_ch), src, 16);
+      }
+      ++ld_kt;
+      if (++ld_c == gm.cin_chunks) {
+        ld_c = 0;
+        if (++ld_kw == gm.KW) { ld_kw = 0; ++ld_kh; }
+      }
+    };
+
+#pragma unroll
+    for (int s = 0; s < STAGES - 1; ++s) {
+      if (s < KT) load_tile(s);
+      cp_async_commit();
     }
-    ++ld_kt;
-    if (++ld_c == p.cin_chunks) {
-      ld_c = 0;
-      if (++ld_kw == p.KW) { ld_kw = 0; ++ld_kh; }
-    }
-  };
 
-  int32_t acc[2][NT][4];
-#pragma unroll
-  for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-    for (int ni = 0; ni < NT; ++ni)
-#pragma unroll
-      for (int k = 0; k < 4; ++k) acc[mi][ni][k] = 0;
+    for (int kt = 0; kt < KT; ++kt) {
+      cp_async_wait<STAGES - 2>();
+      fence_proxy_async_smem();   // this thread's cp.async data -> visible to wgmma (async proxy)
+      __syncthreads();            // every thread's data has landed; every warpgroup finished reading the stage refilled below
+      if (kt + STAGES - 1 < KT) load_tile((kt + STAGES - 1) % STAGES);
+      cp_async_commit();
 
+      const int stage = kt % STAGES;
+      const uint32_t a_base = smem_u32(sA + stage * S::A_STAGE);
+      const uint32_t b_base = smem_u32(sB + stage * S::B_STAGE);
 #pragma unroll
-  for (int s = 0; s < STAGES - 1; ++s) {
-    if (s < KT) load_tile(s);
-    cp_async_commit();
-  }
-
-  for (int kt = 0; kt < KT; ++kt) {
-    cp_async_wait<STAGES - 2>();
-    __syncthreads();
-    if (kt + STAGES - 1 < KT) load_tile((kt + STAGES - 1) % STAGES);
-    cp_async_commit();
-
-    const int stage = kt % STAGES;
-    const uint32_t a_base = smem_u32(sA + stage * S::A_STAGE);
-    const uint32_t b_base = smem_u32(sB + stage * S::B_STAGE);
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
-      uint32_t af[2][4];
-#pragma unroll
-      for (int mi = 0; mi < 2; ++mi) {
-        const int row = wm * 32 + mi * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+      for (int ks = 0; ks < 2; ++ks) {   // two k32 steps per 64-channel k-tile
+        const uint64_t bdesc = wgmma_desc_sw64(b_base + ks * 32);
         if constexpr (!A4) {
-          ldmatrix_x4(af[mi][0], af[mi][1], af[mi][2], af[mi][3], a_base + swz<64>(row, ks * 2 + (lane >> 4)));
+          wgmma_fence();
+          wgmma_ss<BN>(acc, wgmma_desc_sw64(a_base + wg * 64 * A_ROW + ks * 32), bdesc);
         } else {
           uint32_t r0, r1;
+          const int row = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
           ldmatrix_x2(r0, r1, a_base + swz<32>(row, ks));
-          af[mi][0] = r0 & 0x0F0F0F0Fu;
-          af[mi][1] = r1 & 0x0F0F0F0Fu;
-          af[mi][2] = (r0 >> 4) & 0x0F0F0F0Fu;
-          af[mi][3] = (r1 >> 4) & 0x0F0F0F0Fu;
+          const uint32_t af[4] = {r0 & 0x0F0F0F0Fu, r1 & 0x0F0F0F0Fu, (r0 >> 4) & 0x0F0F0F0Fu, (r1 >> 4) & 0x0F0F0F0Fu};
+          wgmma_fence();
+          wgmma_rs<BN>(acc, af, bdesc);
         }
       }
-      uint32_t bf[NT][2];
-#pragma unroll
-      for (int nj = 0; nj < NT / 2; ++nj) {
-        const int row = wn * WNT + nj * 16 + (lane & 7) + (lane >> 4) * 8;
-        ldmatrix_x4(bf[2 * nj][0], bf[2 * nj][1], bf[2 * nj + 1][0], bf[2 * nj + 1][1],
-                    b_base + swz<64>(row, ks * 2 + ((lane >> 3) & 1)));
-      }
-#pragma unroll
-      for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-        for (int ni = 0; ni < NT; ++ni) mma_16832<A4>(acc[mi][ni], af[mi], bf[ni]);
+      wgmma_commit();
+      wgmma_wait_all();
+      fence_operands(acc);
     }
-  }
-  cp_async_wait<0>();
-  __syncthreads();   // pipeline buffers are free: reused for the residual tile (RESIDUAL epilogue)
+    cp_async_wait<0>();
+    __syncthreads();   // pipeline buffers are free
+  };
 
-  // RESIDUAL: bulk-load this tile of the residual operand (coalesced 16 B cp.async, zero-fill past M) instead of
-  // issuing dependent scalar loads inside the epilogue; padded pitch keeps the fragment-pattern reads conflict-free.
-  uint8_t* sRes = smem;
+  // RESIDUAL operand tile in shared memory; padded pitch keeps the fragment-pattern reads conflict-free
+  uint8_t* sRes = smem + S::RES_OFF;
   const int res_es = (p.mode == HAWQ_EPI_RESIDUAL) ? ((p.res_kind == 1 || p.res_bits == 32) ? 4 : 2) : 0;
   const int res_pitch = BN * res_es + 8 * res_es;
-  if (res_es) {
+
+  if constexpr (DUAL) {   // identity convolution first: acc + bias2 (saturating) is the int32 res_kind 1 operand
+    gemm(ConvGeom{p.x2, p.w2, p.H2, p.W2, p.stride2, 0, 1, 1, p.cin_chunks2, p.x2_pix_bytes, p.cin_chunks2 * 64});
+#pragma unroll
+    for (int ni = 0; ni < NT; ++ni) {
+      const int col = ni * 8 + 2 * t;
+      const int b0 = sResChan[col].bias, b1 = sResChan[col + 1].bias;
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        const int row = warp * 16 + hf * 8 + g;
+        *reinterpret_cast<int2*>(sRes + row * res_pitch + col * 4) =
+            make_int2(sat_add(acc[ni * 4 + hf * 2], b0), sat_add(acc[ni * 4 + hf * 2 + 1], b1));
+      }
+    }
+  }
+  gemm(ConvGeom{p.x, p.w, p.H, p.W, p.stride, p.pad, p.KH, p.KW, p.cin_chunks, p.x_pix_bytes, p.K});
+
+  // RESIDUAL: bulk-load this tile of the residual operand (coalesced 16 B cp.async, zero-fill past M) instead of
+  // issuing dependent scalar loads inside the epilogue.
+  if (!DUAL && res_es) {
     const int cpr = BN * res_es / 16;   // 16-byte chunks per row
     const uint8_t* gres = reinterpret_cast<const uint8_t*>(p.res);
     for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
@@ -271,16 +292,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       const int lo = p.relu ? max(p.lo, 0) : p.lo, hi = p.hi;
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
-        const int col = wn * WNT + ni * 8 + 2 * t;
+        const int col = ni * 8 + 2 * t;
         const double2 Cb = *reinterpret_cast<const double2*>(&sCb[col]);
         const double2 M = *reinterpret_cast<const double2*>(&sM[col]);
-#pragma unroll
-        for (int mi = 0; mi < 2; ++mi) {
+        {
 #pragma unroll
           for (int hf = 0; hf < 2; ++hf) {
-            const int row = wm * 32 + mi * 16 + hf * 8 + g;
-            const double d0 = __hiloint2double(0x43300000, acc[mi][ni][hf * 2 + 0] ^ 0x80000000) - Cb.x;
-            const double d1 = __hiloint2double(0x43300000, acc[mi][ni][hf * 2 + 1] ^ 0x80000000) - Cb.y;
+            const int row = warp * 16 + hf * 8 + g;
+            const double d0 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 0] ^ 0x80000000) - Cb.x;
+            const double d1 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 1] ^ 0x80000000) - Cb.y;
             const int q0 = clampi(__double2loint(__fma_rn(d0, M.x, kMagic)), lo, hi);
             const int q1 = clampi(__double2loint(__fma_rn(d1, M.y, kMagic)), lo, hi);
             *reinterpret_cast<uint16_t*>(sOut + row * S::OUT_PITCH + col) = (uint16_t)__byte_perm(q0, q1, 0x0040);
@@ -291,27 +311,38 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   }
 
   if constexpr (EPI == EPI_FAST_RES) {
-    if (!use_slow) {
+    if (!use_slow || use_wide) {
       fast_done = true;
+      // t = fma(d, M, 1.5 * 2^52) with d * M exact inside the FMA: for |d * M| < 2^51 the low word of t is RHE(d * M); a term outside
+      // int32 (which includes every |d * M| >= 2^51) is detected on t - 1.5 * 2^52 (exact in range, far out of range otherwise)
+      bool ovf = false;
+      auto term = [&](double d, double Mx, bool row_ok) -> int {
+        const double tt = __fma_rn(d, Mx, kMagic);
+        if (use_wide) {
+          const double q = tt - kMagic;
+          ovf |= row_ok && (q > 2147483647.0 || q < -2147483648.0);
+        }
+        return __double2loint(tt);
+      };
       const double res_M = dyadic_to_double(p.res_m, p.res_e), low_M = dyadic_to_double(p.low_m, p.low_e);
       const int relu_floor = p.relu ? 0 : (int)0x80000000;
       int ymax = 0;
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
-        const int col = wn * WNT + ni * 8 + 2 * t;
+        const int col = ni * 8 + 2 * t;
         const double2 Cb = *reinterpret_cast<const double2*>(&sCb[col]);
         const double2 M = *reinterpret_cast<const double2*>(&sM[col]);
         double2 M1 = make_double2(res_M, res_M);
         if (p.res_kind == 1) M1 = *reinterpret_cast<const double2*>(&sM1[col]);
-#pragma unroll
-        for (int mi = 0; mi < 2; ++mi) {
+        {
 #pragma unroll
           for (int hf = 0; hf < 2; ++hf) {
-            const int row = wm * 32 + mi * 16 + hf * 8 + g;
-            const double d0 = __hiloint2double(0x43300000, acc[mi][ni][hf * 2 + 0] ^ 0x80000000) - Cb.x;
-            const double d1 = __hiloint2double(0x43300000, acc[mi][ni][hf * 2 + 1] ^ 0x80000000) - Cb.y;
-            const int v0 = __double2loint(__fma_rn(d0, M.x, kMagic));
-            const int v1 = __double2loint(__fma_rn(d1, M.y, kMagic));
+            const int row = warp * 16 + hf * 8 + g;
+            const bool row_ok = m0 + row < p.M;
+            const double d0 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 0] ^ 0x80000000) - Cb.x;
+            const double d1 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 1] ^ 0x80000000) - Cb.y;
+            const int v0 = term(d0, M.x, row_ok);
+            const int v1 = term(d1, M.y, row_ok);
             uint8_t* rptr = sRes + row * res_pitch + col * res_es;
             double r0, r1;
             if (res_es == 2) {   // uint16 residual stream: non-negative, no sign fix-up
@@ -323,10 +354,10 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
               r0 = __hiloint2double(0x43300000, pr.x ^ 0x80000000) - kOffS;
               r1 = __hiloint2double(0x43300000, pr.y ^ 0x80000000) - kOffS;
             }
-            int y0 = max(sat_add(__double2loint(__fma_rn(r0, M1.x, kMagic)), v0), relu_floor);
-            int y1 = max(sat_add(__double2loint(__fma_rn(r1, M1.y, kMagic)), v1), relu_floor);
+            int y0 = max(sat_add(term(r0, M1.x, row_ok), v0), relu_floor);
+            int y1 = max(sat_add(term(r1, M1.y, row_ok), v1), relu_floor);
             if (p.y_bits == 16) {
-              ymax = max(ymax, max(y0, y1));
+              if (row_ok) ymax = max(ymax, max(y0, y1));
               const uint32_t packed = (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
               if (y_in_place) *reinterpret_cast<uint32_t*>(rptr) = packed;
               else if (m0 + row < p.M)
@@ -347,6 +378,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
         }
       }
       if (p.y_bits == 16 && ymax > 65535) atomicOr(p.status, HAWQ_FLAG_RESIDUAL_OVERFLOW);
+      if (ovf) atomicOr(p.status, HAWQ_FLAG_REQUANT_OVERFLOW);
     }
   }
 
@@ -357,21 +389,32 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       if constexpr (FAST) return rhe_requant_fast(v, M);
       else return rhe_requant(v, m, e);
     };
-#pragma unroll
-    for (int mi = 0; mi < 2; ++mi) {
+    // the two terms of a RESIDUAL sum: under a ratio promise (check_ovf) a term outside int32 raises HAWQ_FLAG_REQUANT_OVERFLOW
+    // (ratios <= 1, the FAST case, cannot leave int32)
+    bool ovf = false;
+    auto rq_term = [&](int32_t v, uint32_t m, int e, double M, bool row_ok) -> int32_t {
+      if constexpr (FAST) {
+        return rhe_requant_fast(v, M);
+      } else {
+        const long long q = rhe_requant64(v, m, e);
+        ovf |= row_ok && (q > 2147483647ll || q < -2147483648ll);
+        return sat_i32(q);
+      }
+    };
+    {
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
-        const int row = wm * 32 + mi * 16 + hf * 8 + g;
+        const int row = warp * 16 + hf * 8 + g;
         const int m = m0 + row;
         const bool ok = m < p.M;
 #pragma unroll
         for (int ni = 0; ni < NT; ++ni) {
-          const int col = wn * WNT + ni * 8 + 2 * t;
+          const int col = ni * 8 + 2 * t;
           const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);
           const int4 c1 = *reinterpret_cast<const int4*>(&sChan[col + 1]);
           const double2 M01 = *reinterpret_cast<const double2*>(&sM[col]);
-          int32_t v0 = sat_add(acc[mi][ni][hf * 2 + 0], c0.x);
-          int32_t v1 = sat_add(acc[mi][ni][hf * 2 + 1], c1.x);
+          int32_t v0 = sat_add(acc[ni * 4 + hf * 2 + 0], c0.x);
+          int32_t v1 = sat_add(acc[ni * 4 + hf * 2 + 1], c1.x);
           const size_t gidx = (size_t)m * p.Cout + n0 + col;
           if (p.mode == HAWQ_EPI_REQUANT) {
             if (p.relu) { v0 = max(v0, 0); v1 = max(v1, 0); }
@@ -410,8 +453,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
                 rm0 = sResChan[col].m; re0 = sResChan[col].e; rm1 = sResChan[col + 1].m; re1 = sResChan[col + 1].e;
               }
             }
-            int32_t y0 = sat_add(rq(r0, rm0, re0, rM0), rq(v0, (uint32_t)c0.y, c0.z, M01.x));
-            int32_t y1 = sat_add(rq(r1, rm1, re1, rM1), rq(v1, (uint32_t)c1.y, c1.z, M01.y));
+            int32_t y0 = sat_add(rq_term(r0, rm0, re0, rM0, ok), rq_term(v0, (uint32_t)c0.y, c0.z, M01.x, ok));
+            int32_t y1 = sat_add(rq_term(r1, rm1, re1, rM1, ok), rq_term(v1, (uint32_t)c1.y, c1.z, M01.y, ok));
             if (p.relu) { y0 = max(y0, 0); y1 = max(y1, 0); }
             if (p.y_bits == 32) {
               if (y_in_place) *reinterpret_cast<int2*>(rptr) = make_int2(y0, y1);
@@ -440,6 +483,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
         }
       }
     }
+    if (ovf && p.check_ovf) atomicOr(p.status, HAWQ_FLAG_REQUANT_OVERFLOW);
   };
   if (!fast_done) {
     if (use_slow) epilogue(std::false_type{});

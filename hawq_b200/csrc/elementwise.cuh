@@ -318,4 +318,20 @@ __global__ void __launch_bounds__(256) unpack_i4_kernel(const uint8_t* __restric
   }
 }
 
+// One-time re-tiling of OHWI int8 weights (hawq_conv2d_desc.w_layout 1): block (n_tile, k_tile) = BN rows x 64 bytes, stored
+// contiguously with the SWIZZLE_64B pattern already applied (the shared-memory B tile of conv_igemm.cuh).
+__global__ void __launch_bounds__(256) retile_weights_kernel(const int8_t* __restrict__ w, int Cout, int K, int BN, int8_t* __restrict__ out) {
+  const int kt_total = K / 64;
+  const long long chunks = (long long)Cout * K / 16;
+  for (long long id = blockIdx.x * (long long)blockDim.x + threadIdx.x; id < chunks; id += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(id & 3);
+    const long long rk = id >> 2;                 // (row, k-tile)
+    const int kt = (int)(rk % kt_total);
+    const int row = (int)(rk / kt_total);
+    const int nt = row / BN, r = row % BN;
+    const int4 v = *reinterpret_cast<const int4*>(w + (size_t)row * K + kt * 64 + c * 16);
+    *reinterpret_cast<int4*>(out + ((size_t)nt * kt_total + kt) * BN * 64 + r * 64 + ((c ^ ((r >> 1) & 3)) << 4)) = v;
+  }
+}
+
 }  // namespace hawq

@@ -17,6 +17,48 @@ constexpr int STEM_PH = 2 * STEM_TH + 5;  // 21
 constexpr int STEM_PW = 2 * STEM_TW + 6;  // 38 (one extra column for the zero-weight 8th tap)
 constexpr int STEM_WPITCH = 60;           // words per output channel in smem (7*8 = 56, padded: conflict-free)
 
+// input patch of one 8x16 output tile (origin iy0, ix0 may lie outside the image: zero fill), one word per pixel
+__device__ __forceinline__ void stem_load_patch(const int8_t* __restrict__ x, int n, int H, int W, int iy0, int ix0, uint32_t* sPatch) {
+  for (int i = threadIdx.x; i < STEM_PH * STEM_PW; i += 256) {
+    const int py = i / STEM_PW, px = i - py * STEM_PW;
+    const int iy = iy0 + py, ix = ix0 + px;
+    uint32_t v = 0;
+    if ((unsigned)iy < (unsigned)H && (unsigned)ix < (unsigned)W) {
+      const int8_t* s = x + ((size_t)(n * H + iy) * W + ix) * 3;
+      v = (uint32_t)(uint8_t)s[0] | ((uint32_t)(uint8_t)s[1] << 8) | ((uint32_t)(uint8_t)s[2] << 16);
+    }
+    sPatch[i] = v;
+  }
+}
+
+// raw accumulators of the 8x16 tile: warp w owns output row w; acc[j] = mma.m16n8 fragment of channels 8j..8j+7
+// (fragment row g / g+8 = output column g / g+8)
+__device__ __forceinline__ void stem_tile_mma(const uint32_t* sPatch, const uint32_t* sW, int32_t (&acc)[8][4]) {
+  const int lane = threadIdx.x & 31, oy = threadIdx.x >> 5;
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) acc[j][k] = 0;
+#pragma unroll
+  for (int kh = 0; kh < 7; ++kh) {
+    const uint32_t* prow = sPatch + (2 * oy + kh) * STEM_PW;
+    uint32_t a[4];
+    a[0] = prow[2 * g + t];
+    a[1] = prow[2 * (g + 8) + t];
+    a[2] = prow[2 * g + 4 + t];
+    a[3] = prow[2 * (g + 8) + 4 + t];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      uint32_t b[2];
+      const uint32_t* wr = sW + (8 * j + g) * STEM_WPITCH + kh * 8;
+      b[0] = wr[t];
+      b[1] = wr[4 + t];
+      mma_16832<false>(acc[j], a, b);
+    }
+  }
+}
+
 // tile loop of the persistent stem variant: gridDim.x CTAs, tile = (n, tile_y, tile_x) with x fastest
 __device__ __forceinline__ void stem_conv_persistent_body(const int8_t* __restrict__ x, const uint32_t* __restrict__ w,
                                                           const hawq_chan* __restrict__ chan, int N, int H, int W, int Ho, int Wo,
@@ -42,40 +84,11 @@ __device__ __forceinline__ void stem_conv_persistent_body(const int8_t* __restri
     const int oy0 = ty * STEM_TH, ox0 = tx * STEM_TW;
     const int iy0 = oy0 * 2 - 3, ix0 = ox0 * 2 - 3;
     __syncthreads();                                   // the previous tile's patch has been consumed
-    for (int i = tid; i < STEM_PH * STEM_PW; i += 256) {
-      const int py = i / STEM_PW, px = i - py * STEM_PW;
-      const int iy = iy0 + py, ix = ix0 + px;
-      uint32_t v = 0;
-      if ((unsigned)iy < (unsigned)H && (unsigned)ix < (unsigned)W) {
-        const int8_t* s = x + ((size_t)(n * H + iy) * W + ix) * 3;
-        v = (uint32_t)(uint8_t)s[0] | ((uint32_t)(uint8_t)s[1] << 8) | ((uint32_t)(uint8_t)s[2] << 16);
-      }
-      sPatch[i] = v;
-    }
+    stem_load_patch(x, n, H, W, iy0, ix0, sPatch);
     __syncthreads();
     int32_t acc[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-      for (int k = 0; k < 4; ++k) acc[j][k] = 0;
+    stem_tile_mma(sPatch, sW, acc);
     const int oy = warp;
-#pragma unroll
-    for (int kh = 0; kh < 7; ++kh) {
-      const uint32_t* prow = sPatch + (2 * oy + kh) * STEM_PW;
-      uint32_t a[4];
-      a[0] = prow[2 * g + t];
-      a[1] = prow[2 * (g + 8) + t];
-      a[2] = prow[2 * g + 4 + t];
-      a[3] = prow[2 * (g + 8) + 4 + t];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        uint32_t b[2];
-        const uint32_t* wr = sW + (8 * j + g) * STEM_WPITCH + kh * 8;
-        b[0] = wr[t];
-        b[1] = wr[4 + t];
-        mma_16832<false>(acc[j], a, b);
-      }
-    }
     const int oyg = oy0 + oy;
     if (oyg >= Ho) continue;                           // (the barriers at the loop top are reached by every thread: no early exit)
 #pragma unroll
@@ -117,6 +130,38 @@ __global__ void __launch_bounds__(256) stem_conv_kernel(const int8_t* __restrict
   stem_conv_persistent_body(x, w, chan, N, H, W, Ho, Wo, lo, hi, out, sPatch, sW, sChan, sM);
 }
 
+// one pooled pixel x 8 channels (max of non-negative int16 values): residual stream y (uint16 / int32, 0 = none) and the
+// first unit's quant_act output (case 0 with scalar m, e; int8 or packed nibbles, 0 = none)
+__device__ __forceinline__ void pool_store(uint4 mx, size_t oidx, int y_bits, void* __restrict__ y, int low_bits, uint32_t low_m, int low_e,
+                                           int low_lo, int low_hi, void* __restrict__ out_low) {
+  int32_t v[8] = {(int)(mx.x & 0xFFFF), (int)(mx.x >> 16), (int)(mx.y & 0xFFFF), (int)(mx.y >> 16),
+                  (int)(mx.z & 0xFFFF), (int)(mx.z >> 16), (int)(mx.w & 0xFFFF), (int)(mx.w >> 16)};
+  if (y_bits == 16) {
+    *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(y) + oidx) = mx;
+  } else if (y_bits == 32) {
+    int32_t* yo = reinterpret_cast<int32_t*>(y) + oidx;
+    *reinterpret_cast<int4*>(yo) = make_int4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<int4*>(yo + 4) = make_int4(v[4], v[5], v[6], v[7]);
+  }
+  if (low_bits != 0) {
+    uint32_t wlo = 0, whi = 0;
+    const bool fast = dyadic_is_fast(low_m, low_e);
+    const double low_M = dyadic_to_double(low_m, low_e);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int32_t qa = fast ? rhe_requant_fast(v[k], low_M) : rhe_requant(v[k], low_m, low_e);
+      const int32_t qb = fast ? rhe_requant_fast(v[k + 4], low_M) : rhe_requant(v[k + 4], low_m, low_e);
+      wlo |= (uint32_t)(clampi(qa, low_lo, low_hi) & 0xFF) << (8 * k);
+      whi |= (uint32_t)(clampi(qb, low_lo, low_hi) & 0xFF) << (8 * k);
+    }
+    if (low_bits == 8) {
+      *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(out_low) + oidx) = make_uint2(wlo, whi);
+    } else {
+      *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(out_low) + (oidx >> 1)) = pack_nibbles8(wlo, whi);
+    }
+  }
+}
+
 // nn.MaxPool2d(3, 2, 1) on the (non-negative) int16 stem output, then: residual stream y (uint16 / int32) and the
 // first unit's quant_act output (case 0 with scalar m, e).  One thread = one output pixel x 8 channels.
 __global__ void __launch_bounds__(256) maxpool_requant_kernel(const int16_t* __restrict__ x, int N, int H, int W, int C,
@@ -149,32 +194,89 @@ __global__ void __launch_bounds__(256) maxpool_requant_kernel(const int16_t* __r
         mx.w = __vmaxs2(mx.w, v.w);
       }
     }
-    const size_t oidx = ((size_t)(n * Ho + ho) * Wo + wo) * C + cg * 8;
-    int32_t v[8] = {(int)(mx.x & 0xFFFF), (int)(mx.x >> 16), (int)(mx.y & 0xFFFF), (int)(mx.y >> 16),
-                    (int)(mx.z & 0xFFFF), (int)(mx.z >> 16), (int)(mx.w & 0xFFFF), (int)(mx.w >> 16)};
-    if (y_bits == 16) {
-      *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(y) + oidx) = mx;
-    } else if (y_bits == 32) {
-      int32_t* yo = reinterpret_cast<int32_t*>(y) + oidx;
-      *reinterpret_cast<int4*>(yo) = make_int4(v[0], v[1], v[2], v[3]);
-      *reinterpret_cast<int4*>(yo + 4) = make_int4(v[4], v[5], v[6], v[7]);
-    }
-    if (low_bits != 0) {
-      uint32_t wlo = 0, whi = 0;
-      const bool fast = dyadic_is_fast(low_m, low_e);
-      const double low_M = dyadic_to_double(low_m, low_e);
+    pool_store(mx, ((size_t)(n * Ho + ho) * Wo + wo) * C + cg * 8, y_bits, y, low_bits, low_m, low_e, low_lo, low_hi, out_low);
+  }
+}
+
+// Fused stem (hawq_stem_pool_i8): convolution + bias + 16-bit requant + ReLU, max-pool 3x3/2, residual-stream store and low-bit
+// copy in one kernel; the int16 convolution output only exists in shared memory.  Persistent CTAs loop over tiles of 3 x 7 pooled
+// pixels, whose 3x3 windows cover the 7 x 15 convolution outputs starting at (2 * py0 - 1, 2 * px0 - 1): one 8x16 tile of the
+// convolution above.  Positions outside the convolution output hold 0, neutral for the max of non-negative values.
+constexpr int STEMP_PH = 3, STEMP_PW = 7;
+__global__ void __launch_bounds__(256) stem_pool_kernel(const int8_t* __restrict__ x, const uint32_t* __restrict__ w256,
+                                                        const hawq_chan* __restrict__ chan, int N, int H, int W, int Ho, int Wo,
+                                                        int Po, int Qo, int lo, int hi, int y_bits, void* __restrict__ y, int low_bits,
+                                                        uint32_t low_m, int low_e, int low_lo, int low_hi, void* __restrict__ out_low) {
+  __shared__ uint32_t sPatch[STEM_PH * STEM_PW];
+  __shared__ uint32_t sW[64 * STEM_WPITCH];
+  __shared__ hawq_chan sChan[64];
+  __shared__ double sM[64];
+  __shared__ __align__(16) int16_t sConv[STEM_TH][STEM_TW][64];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, t = lane & 3;
+  for (int i = tid; i < 64 * 56; i += 256) sW[(i / 56) * STEM_WPITCH + (i % 56)] = w256[(i / 56) * 64 + (i % 56)];   // kernel rows 0..6
+  int slow = 0;
+  if (tid < 64) {
+    const hawq_chan c = chan[tid];
+    sChan[tid] = c;
+    sM[tid] = dyadic_to_double(c.m, c.e);
+    slow = !dyadic_is_fast(c.m, c.e);
+  }
+  const bool use_slow = __syncthreads_or(slow) != 0;
+  const int tiles_x = (Qo + STEMP_PW - 1) / STEMP_PW, tiles_y = (Po + STEMP_PH - 1) / STEMP_PH;
+  const long long total = (long long)N * tiles_y * tiles_x;
+  for (long long tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    const int tx = (int)(tile % tiles_x);
+    const int ty = (int)((tile / tiles_x) % tiles_y);
+    const int n = (int)(tile / ((long long)tiles_x * tiles_y));
+    const int py0 = ty * STEMP_PH, px0 = tx * STEMP_PW;
+    const int oy0 = 2 * py0 - 1, ox0 = 2 * px0 - 1;
+    __syncthreads();                                   // the previous tile's patch and convolution tile have been consumed
+    stem_load_patch(x, n, H, W, oy0 * 2 - 3, ox0 * 2 - 3, sPatch);
+    __syncthreads();
+    int32_t acc[8][4];
+    stem_tile_mma(sPatch, sW, acc);
+    const int oyg = oy0 + warp;
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int32_t qa = fast ? rhe_requant_fast(v[k], low_M) : rhe_requant(v[k], low_m, low_e);
-        const int32_t qb = fast ? rhe_requant_fast(v[k + 4], low_M) : rhe_requant(v[k + 4], low_m, low_e);
-        wlo |= (uint32_t)(clampi(qa, low_lo, low_hi) & 0xFF) << (8 * k);
-        whi |= (uint32_t)(clampi(qb, low_lo, low_hi) & 0xFF) << (8 * k);
+    for (int hf = 0; hf < 2; ++hf) {
+      const int cx = g + hf * 8, oxg = ox0 + cx;
+      const bool ok = (unsigned)oyg < (unsigned)Ho && (unsigned)oxg < (unsigned)Wo;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int c = 8 * j + 2 * t;
+        const hawq_chan c0 = sChan[c], c1 = sChan[c + 1];
+        const int32_t v0 = sat_add(acc[j][hf * 2 + 0], c0.bias), v1 = sat_add(acc[j][hf * 2 + 1], c1.bias);
+        int32_t q0, q1;
+        if (use_slow) {
+          q0 = rhe_requant(v0, c0.m, c0.e);
+          q1 = rhe_requant(v1, c1.m, c1.e);
+        } else {
+          q0 = rhe_requant_fast(v0, sM[c]);
+          q1 = rhe_requant_fast(v1, sM[c + 1]);
+        }
+        q0 = ok ? max(clampi(q0, lo, hi), 0) : 0;
+        q1 = ok ? max(clampi(q1, lo, hi), 0) : 0;
+        *reinterpret_cast<uint32_t*>(&sConv[warp][cx][c]) = (uint32_t)(q0 & 0xFFFF) | ((uint32_t)(q1 & 0xFFFF) << 16);
       }
-      if (low_bits == 8) {
-        *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(out_low) + oidx) = make_uint2(wlo, whi);
-      } else {
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(out_low) + (oidx >> 1)) = pack_nibbles8(wlo, whi);
-      }
+    }
+    __syncthreads();
+    for (int i = tid; i < STEMP_PH * STEMP_PW * 8; i += 256) {
+      const int cg = i & 7, pix = i >> 3;
+      const int ry = pix / STEMP_PW, rx = pix - ry * STEMP_PW;
+      const int po = py0 + ry, qo = px0 + rx;
+      if (po >= Po || qo >= Qo) continue;
+      uint4 mx = make_uint4(0, 0, 0, 0);
+#pragma unroll
+      for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 3; ++dx) {
+          const uint4 v = *reinterpret_cast<const uint4*>(&sConv[2 * ry + dy][2 * rx + dx][cg * 8]);
+          mx.x = __vmaxs2(mx.x, v.x);
+          mx.y = __vmaxs2(mx.y, v.y);
+          mx.z = __vmaxs2(mx.z, v.z);
+          mx.w = __vmaxs2(mx.w, v.w);
+        }
+      pool_store(mx, ((size_t)(n * Po + po) * Qo + qo) * 64 + cg * 8, y_bits, y, low_bits, low_m, low_e, low_lo, low_hi, out_low);
     }
   }
 }

@@ -7,7 +7,7 @@ to the unit's first convolution (they read the same activation).  With a single 
 it to GLPK through pulp, neither of which is available here, so :func:`solve` is a small exact branch-and-bound (fractional-knapsack
 bound).  ``layer_order`` / ``tie_pairs`` give the reference's variable numbering so results map onto ``bit_config.py`` entries, and
 :func:`latency_table_from_detail` turns per-launch timings of this engine (``bench.py --detail``) into the ``latency_int4`` /
-``latency_int8`` arrays the notebook expects, i.e. the B200 replacement of the reference's T4 table (ILP.ipynb cells 4 / 17).
+``latency_int8`` arrays the notebook expects, i.e. this engine's replacement of the reference's T4 table (ILP.ipynb cells 4 / 17).
 """
 import numpy as np
 
@@ -55,7 +55,7 @@ def solve(sensitivity, cost4, cost8, limit, ties=()):
     weight = np.array([(c8 - c4)[[i for i in range(n) if group[i] == g]].sum() for g in reps])     # cost of going to 8 bit
     cap = float(limit) - float(c4.sum())
     take = np.zeros(len(reps), dtype=bool)
-    free = (weight <= 0) & (value >= 0)                # 8 bit is no more expensive than 4 bit (e.g. this engine's 4-bit layers on B200): take
+    free = (weight <= 0) & (value >= 0)                # 8 bit is no more expensive than 4 bit (e.g. this engine's 4-bit layers, which run on int8 MMA): take
     if cap - float(weight[free].sum()) < -1e-9:
         raise ValueError("infeasible: the budget is below the cheapest assignment")
     order = [i for i in np.argsort(-(value / np.maximum(weight, 1e-300))) if not free[i] and value[i] > 0]

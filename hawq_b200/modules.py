@@ -7,7 +7,7 @@ Two regimes, chosen exactly like the reference does (``fix_flag`` / ``running_st
 
 * un-frozen: float "fake-quant" arithmetic in torch (``quant_math``) — this is the calibration / QAT-side behaviour
   (range statistics are updated); it is not the product's hot path.
-* frozen (after ``freeze_model``): integer-only execution on the B200 kernels behind the C ABI.  A frozen module
+* frozen (after ``freeze_model``): integer-only execution on the H100 kernels behind the C ABI.  A frozen module
   accepts an ``IntActivation`` payload from the previous engine module (no fp32 round trip) or a CUDA fp32
   tensor at a graph edge; there is no CPU or PyTorch fallback — a frozen forward without CUDA raises.
   ``hawq_b200.compile_model`` turns a whole frozen graph into a fused plan replayed as one CUDA graph.

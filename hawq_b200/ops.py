@@ -96,7 +96,7 @@ def conv_desc(N, H, W, Cin, Cout, kh, kw, stride, pad, a_bits, w_layout=0):
 
 
 def upload_weights(w_ohwi_cpu, device):
-    """int8 OHWI host weights -> device buffer [OHWI | tcgen05 re-tiled copy] (hawq_conv_desc.w_layout = 1)."""
+    """int8 OHWI host weights -> device buffer [OHWI | re-tiled copy] (hawq_conv_desc.w_layout = 1)."""
     cout = w_ohwi_cpu.shape[0]
     k = w_ohwi_cpu.numel() // cout
     buf = torch.empty(2 * cout * k, dtype=torch.int8, device=device)
@@ -135,12 +135,10 @@ def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None,
     h, s = _ctx(x)
     ev = _begin()
     lib = _lib.load()
-    halo0, c10 = (lib.hawq_debug_kernel_count(1), lib.hawq_debug_kernel_count(3)) if ev is not None else (0, 0)
     _lib.check(lib.hawq_conv2d(h, C.byref(desc), C.byref(ep), _p(x), _p(w), _p(chan), _p(res), _p(res_chan),
                                _p(fscale), _p(out), _p(out_low), s))
-    if ev is not None:     # per-launch timing (bench.py roofline leg): name the kernel family that took the launch
-        name = "conv_halo" if lib.hawq_debug_kernel_count(1) != halo0 else "conv1x1" if lib.hawq_debug_kernel_count(3) != c10 else "conv_tc"
-        _count(name, conv_work(desc, ep), ev)
+    if ev is not None:     # per-launch timing (bench.py roofline leg)
+        _count("conv_igemm", conv_work(desc, ep), ev)
     else:
         _count()
 
@@ -149,7 +147,6 @@ def conv2d_dual(x, desc, ep, w, chan, desc2, x2, w2, chan2, out=None, out_low=No
     """resize unit: identity 1x1 conv (desc2/x2/w2/chan2) + last 1x1 conv (desc/x/w/chan) + case-1 sum in one kernel."""
     h, s = _ctx(x)
     ev = _begin()
-    k0 = _lib.load().hawq_debug_kernel_count(4) if ev is not None else 0
     _lib.check(_lib.load().hawq_conv2d_dual(h, C.byref(desc), C.byref(ep), _p(x), _p(w), _p(chan), C.byref(desc2), _p(x2), _p(w2),
                                             _p(chan2), _p(out), _p(out_low), s))
     work = None
@@ -159,7 +156,7 @@ def conv2d_dual(x, desc, ep, w, chan, desc2, x2, w2, chan2, out=None, out_low=No
         b = (m * (desc.Cin + desc2.Cin) * desc.a_bits // 8 + desc.Cout * (desc.Cin + desc2.Cin) + 32 * desc.Cout
              + m * desc.Cout * (ep.y_bits + ep.low_bits) // 8)
         work = (macs, b)
-    _count("conv_dual" if ev is not None and _lib.load().hawq_debug_kernel_count(4) != k0 else "conv_tc_dual", work, ev)
+    _count("conv_dual", work, ev)
 
 
 def linear(x, w, chan, fscale, out, n, k, cout, cout_pad):
@@ -186,7 +183,7 @@ def stem_pool(x, w256, chan, clamp, n, hh, ww, y_bits, y, low_bits, low_me, low_
                                              low_me[1], low_clamp[0], low_clamp[1], _p(out_low), s))
     ho, wo = (hh - 1) // 2 + 1, (ww - 1) // 2 + 1
     po, qo = (ho - 1) // 2 + 1, (wo - 1) // 2 + 1
-    _count("stem_tc", (n * ho * wo * 64 * 147, n * hh * ww * 3 + 64 * 256 + 1024 + n * po * qo * 64 * (y_bits + low_bits) // 8) if ev is not None else None, ev)
+    _count("stem_pool", (n * ho * wo * 64 * 147, n * hh * ww * 3 + 64 * 256 + 1024 + n * po * qo * 64 * (y_bits + low_bits) // 8) if ev is not None else None, ev)
 
 
 def maxpool_requant(x, n, hh, ww, c, y_bits, y, low_bits, low_me, low_clamp, out_low):

@@ -37,10 +37,10 @@ class EngineConfig(threading.local):
     residual_bits = 32
     fast_kernels = True
     checked = False
-    # HBM container of 4-bit activations: 8 = one value per byte (the int8 kernels consume them directly: Blackwell has no int4 MMA,
-    # so packed nibbles must be expanded on chip before every use), 4 = packed nibbles (half the bytes of those tensors, expansion by
-    # converter warps).  Same integers either way; today the byte container is faster on every ResNet layer (profiles/r02), the
-    # packed one is kept for bandwidth-bound deployments and is what the kernel tests exercise with a_bits = 4.
+    # HBM container of 4-bit activations: 8 = one value per byte (the int8 kernels consume them directly: Hopper has no int4 MMA,
+    # so packed nibbles must be expanded on chip before every use), 4 = packed nibbles (half the bytes of those tensors, expanded in
+    # registers by the convolution).  Same integers either way; the byte container is the default, the packed one is kept for
+    # bandwidth-bound deployments and is what the kernel tests exercise with a_bits = 4.
     a4_container = 4 if os.environ.get("HAWQ_B200_A4_STORAGE", "byte") == "packed" else 8
     dual = os.environ.get("HAWQ_B200_DUAL", "1") != "0"   # resize units: identity conv + last conv in one kernel (uint16 stream only)
 
@@ -274,12 +274,10 @@ def _conv_cache(mod, a_sf, a_bits, device):
         w = w_int.detach().to("cpu").permute(0, 2, 3, 1).contiguous().to(torch.int8)      # OHWI
         bias = (b_int.detach().to("cpu").to(torch.int64).numpy() if b_int is not None else np.zeros(cout, dtype=np.int64))
         stem = (cin == 3 and kh == 7 and conv.stride[0] == 2 and conv.padding[0] == 3 and cout == 64)
-        w256 = None
         if stem:
             wp = torch.zeros((cout, 8, 8, 4), dtype=torch.int8)       # kernel rows 7 -> 8, taps 7 -> 8, channels 3 -> 4 (zeros)
             wp[:, :7, :7, :3] = w
-            w256 = wp.to(device)                                      # fused tcgen05 stem: K = 256
-            w = wp[:, :7].contiguous()                                # two-kernel path: K = 224
+            w = wp[:, :7].contiguous()                                # stem kernel layout: K = 224
         else:
             if cin % 64 != 0 or cout % 64 != 0:
                 raise NotImplementedError("hawq_b200 convolutions need Cin and Cout multiples of 64 (got %d, %d)" % (cin, cout))
@@ -287,7 +285,7 @@ def _conv_cache(mod, a_sf, a_bits, device):
                 ops.permute_weights_for_i4(w)
         tiled = (not stem) and torch.device(device).type == "cuda"
         ent = dict(w=ops.upload_weights(w, device) if tiled else w.to(device), w_layout=1 if tiled else 0, w_sf=w_sf, bias=bias, cout=cout, cin=cin, k=kh, stride=conv.stride[0],
-                   pad=conv.padding[0], stem=stem, chan={}, w256=w256)
+                   pad=conv.padding[0], stem=stem, chan={})
     c[key] = ent
     return ent
 
@@ -425,7 +423,7 @@ def _launch_residual(r, low_act, device):
         res_chan = _chan_tensor(ient, _act_tag("c1res", act), m1, e1, device)
         res_kind, res_bits, res_me = 1, 32, (0, 1)
         pairs.append((m1, e1))
-        # resize units: both 1x1 convolutions in one kernel (two TMEM accumulators) when the fast uint16 stream is in use
+        # resize units: both 1x1 convolutions in one kernel when the fast uint16 stream is in use
         if (config.dual and r.relu and config.residual_bits == 16 and ent["k"] == 1 and ent["stride"] == 1 and ent["pad"] == 0
                 and ient["k"] == 1 and ient["pad"] == 0 and ent["w_layout"] == 1 and ient["w_layout"] == 1
                 and conv.src.bits == ident.src.bits):
@@ -504,18 +502,11 @@ def _launch_stem(st, low_act, device):
         low_bits, low_me, low_clamp = _store_bits(low_act), (lm[0], le[0]), _act_clamp(low_act)
         low = _alloc(device, numel, low_bits)
         low_node = Node("int", (nb, 64, po, qo), data=low, bits=low_bits, signed=_store_signed(low_act))
-    fused = False
-    if config.fast_kernels and min(e) >= 31 and (low_bits == 0 or low_me[0] == 0 or 31 <= low_me[1] <= 51):
-        try:                    # one kernel: convolution, pool, requantisation, low-bit copy (the int16 tensor never exists)
-            ops.stem_pool(src.data, ent["w256"], chan, (lo, hi), nb, hh, ww, y_bits, y, low_bits, low_me, low_clamp, low)
-            fused = True
-        except HawqError as err:
-            if err.code != ERR_UNSUPPORTED:
-                raise
-    if not fused:
-        t16 = torch.empty(nb * ho * wo * 64, dtype=torch.int16, device=device)
-        ops.stem_conv(src.data, ent["w"], chan, (lo, hi), t16, nb, hh, ww)
-        ops.maxpool_requant(t16, nb, ho, wo, 64, y_bits, y, low_bits, low_me, low_clamp, low)
+    # two kernels (convolution -> int16, then max-pool + requant): measured faster on H100 than the one-kernel hawq_stem_pool_i8, whose
+    # persistent tiles recompute the overlapping pool windows' convolution outputs (DESIGN.md §6)
+    t16 = torch.empty(nb * ho * wo * 64, dtype=torch.int16, device=device)
+    ops.stem_conv(src.data, ent["w"], chan, (lo, hi), t16, nb, hh, ww)
+    ops.maxpool_requant(t16, nb, ho, wo, 64, y_bits, y, low_bits, low_me, low_clamp, low)
     st.shape = (nb, 64, po, qo)
     st.become_int(y, y_bits, signed=(y_bits == 32))
     return low_node

@@ -1,4 +1,4 @@
-/* hawq_b200.h — C ABI of libhawq_b200.so: the integer forward path of HAWQ-quantized ResNets on B200 (sm_100a).
+/* hawq_b200.h — C ABI of libhawq_b200.so: the integer forward path of HAWQ-quantized ResNets on H100 (sm_90a).
  *
  * The reference (Zhen-Dong/HAWQ) has no FFI / operator-registration layer: its boundary for this path is the Python
  * nn.Module API of utils/quantization_utils/quant_modules.py.  Each entry point below therefore cites the reference
@@ -14,7 +14,7 @@
  *     "hawq nibble order": inside every group of 8 consecutive channels, byte j (0..3) holds channel j in its low
  *     nibble and channel j+4 in its high nibble (so a 32-bit word expands to two int8x4 words with one AND and one
  *     SHIFT+AND).  hawq_pack_i4 / hawq_unpack_i4 convert from/to one-value-per-byte;
- *   - weights are int8, OHWI ([Cout][kh][kw][Cin], K-major) for 8- and 4-bit layers alike (Blackwell has no int4
+ *   - weights are int8, OHWI ([Cout][kh][kw][Cin], K-major) for 8- and 4-bit layers alike (Hopper has no int4
  *     MMA: 4-bit weights are widened once at plan time; they are <1% of the traffic).  For layers whose INPUT is
  *     packed 4-bit the K order inside each 32-channel block must be permuted with hawq_permute_weights_for_i4
  *     (host helper) to match the on-chip nibble expansion;
@@ -98,11 +98,11 @@ typedef struct {
 } hawq_epilogue_desc;
 
 /* Caller promise: every dyadic pair of this launch (chan[], res_chan[], res_m/e, low_m/e) has ratio m * 2^-e <= 1, i.e.
- * e >= 31 or m == 0 (true for every HAWQ ResNet layer).  Enables the tcgen05 kernel, which evaluates RHE(v * m / 2^e) with one
- * exact FP64 FMA.  The kernel re-checks the promise and raises HAWQ_FLAG_BAD_RATIO instead of computing wrong numbers. */
+ * e >= 31 or m == 0 (true for every HAWQ ResNet layer).  The convolution evaluates RHE(v * m / 2^e) with one exact FP64 FMA
+ * when every ratio of the CTA's channels is <= 1 (checked in the kernel) and with the exact 64-bit integer form otherwise. */
 #define HAWQ_EP_RATIOS_LE_ONE 1
-/* Weaker promise: every ratio <= 2^20 (e >= 11 or m == 0).  Same fast kernel plus an exact per-value check that the
- * requantised term fits int32; a violation raises HAWQ_FLAG_REQUANT_OVERFLOW (the generic kernels saturate instead). */
+/* Weaker promise: every ratio <= 2^20 (e >= 11 or m == 0).  Under either promise a RESIDUAL term whose requantised value
+ * leaves int32 raises HAWQ_FLAG_REQUANT_OVERFLOW (without a promise the sum saturates silently, as the reference's int32 cast). */
 #define HAWQ_EP_RATIOS_LE_2P20 2
 
 /* ---- lifetime ---------------------------------------------------------------------------------------------- */
@@ -137,8 +137,8 @@ int hawq_conv2d_i4(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_
                    void* out, void* out_low, void* stream);
 
 /* Resize residual units (Q_ResUnitBn with resize_identity, q_resnet.py:304-330): the identity-branch 1x1 convolution
- * (d2/x2/w2; stride d2->stride, pad 0) and the unit's last 1x1 convolution (d/x/w; stride 1) are accumulated side by side in
- * one kernel and combined by the case-1 fixed-point sum (quant_utils.py:430-456):
+ * (d2/x2/w2; stride d2->stride, pad 0) and the unit's last 1x1 convolution (d/x/w; stride 1) are computed one after the other
+ * in one kernel (the identity result stays in shared memory) and combined by the case-1 fixed-point sum (quant_utils.py:430-456):
  *   y = ReLU( RHE((acc2 + chan2.bias) * chan2.m / 2^chan2.e) + RHE((acc + chan.bias) * chan.m / 2^chan.e) )
  * ep: mode RESIDUAL, relu 1, y_bits 16 (uint16 stream in out), optional low-bit copy in out_low, flags = ratio promise.
  * Both descriptors need w_layout 1 and equal a_bits / Cout / output grids.  Returns HAWQ_ERR_UNSUPPORTED for any other
@@ -161,11 +161,12 @@ int hawq_linear_i8(hawq_handle* h, int32_t N, int32_t K, int32_t Cout, int32_t C
 int hawq_stem_conv_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_t* x, const int8_t* w,
                       const hawq_chan* chan, int32_t clamp_lo, int32_t clamp_hi, int16_t* out, void* stream);
 
-/* Fused stem (tcgen05): quant_init_convbn (7x7 stride 2 pad 3, Cin = 3 -> 64) + nn.MaxPool2d(3, 2, 1) + quant_act_int32 (16-bit dyadic
+/* Fused stem: quant_init_convbn (7x7 stride 2 pad 3, Cin = 3 -> 64) + nn.MaxPool2d(3, 2, 1) + quant_act_int32 (16-bit dyadic
  * requant, clamp) + ReLU, and optionally the first unit's low-bit quant_act (q_resnet.py:117-122, :234) in one kernel; the int16
  * convolution output never reaches HBM.  w256 = int8 [64][8][8][4] (kernel rows padded 7 -> 8, taps 7 -> 8, channels 3 -> 4, zeros
- * in the padding).  y = pooled residual stream [N][Hp][Wp][64] as uint16 (y_bits 16) or int32 (32).  Preconditions: every ratio
- * <= 1, W % 4 == 0, W <= 256; otherwise HAWQ_ERR_UNSUPPORTED (use hawq_stem_conv_i8 + hawq_maxpool_requant: same integers). */
+ * in the padding).  y = pooled residual stream [N][Hp][Wp][64] as uint16 (y_bits 16) or int32 (32).  Preconditions: the ratio
+ * of the low-bit copy <= 1, W % 16 == 0 (row pitch a multiple of 16 bytes), W <= 256; otherwise HAWQ_ERR_UNSUPPORTED (use
+ * hawq_stem_conv_i8 + hawq_maxpool_requant: same integers). */
 int hawq_stem_pool_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_t* x, const int8_t* w256, const hawq_chan* chan,
                       int32_t clamp_lo, int32_t clamp_hi, int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
                       int32_t low_lo, int32_t low_hi, void* out_low, void* stream);
@@ -213,23 +214,16 @@ int hawq_dyadic(double ratio, uint32_t* m, int32_t* e);
 int64_t hawq_rhe_requant_host(int32_t v, uint32_t m, int32_t e);
 /* K permutation inside each 32-channel block for layers whose input is packed 4-bit (in place, int8 OHWI, host memory) */
 int hawq_permute_weights_for_i4(int8_t* host_w, int64_t rows_times_taps, int32_t Cin);
-/* Re-tile int8 OHWI weights [Cout][K] for the tcgen05 convolution: block (n_tile, k_tile) = BN rows x 64 bytes (BN = 128 when
- * Cout % 128 == 0, else 64), stored contiguously with the shared-memory swizzle pre-applied, so the kernel fetches a k-tile of
- * weights with one linear bulk copy.  `out` (Cout * K bytes) is normally w_ohwi + Cout * K, i.e. the copy is appended to the OHWI
+/* Re-tile int8 OHWI weights [Cout][K]: block (n_tile, k_tile) = BN rows x 64 bytes (BN = 128 when Cout % 128 == 0, else 64),
+ * stored contiguously with the shared-memory swizzle pre-applied (a k-tile of weights is one linear copy).  The convolution
+ * kernels of this build read the OHWI part; hawq_conv2d_dual requires the layout.  `out` (Cout * K bytes) is normally w_ohwi + Cout * K, i.e. the copy is appended to the OHWI
  * tensor and announced with hawq_conv_desc.w_layout = 1.  Device pointers, asynchronous on the stream. */
 int hawq_retile_weights(hawq_handle* h, const int8_t* w_ohwi, int32_t Cout, int64_t K, int8_t* out, void* stream);
-/* debug: number of hawq_conv2d launches so far that went to kernel family 0 = conv_tc (generic tcgen05 implicit GEMM),
- * 1 = conv_halo (3x3 stride-1, A operand read in place), 2 = conv_halo launches that needed the 2-D weight-map fallback,
- * 3 = conv1x1 (1x1 stride-1, stationary weights), 4 = conv_dual (resize-unit tail, stationary weights), 5 = resize-unit tails
- * on conv_tc, 6 = fused tcgen05 stem;
+/* debug: number of launches so far by kernel family: 0 = hawq_conv2d (wgmma implicit GEMM), 4 = hawq_conv2d_dual (both
+ * convolutions of a resize-unit tail in one kernel); 6 = hawq_stem_pool_i8 (fused stem); families 1-3, 5 and 7 are unused
+ * in this build and stay 0;
  * -1 for an unknown family.  Lets tests assert which kernel ran. */
 int64_t hawq_debug_kernel_count(int32_t family);
-/* debug: with HAWQ_B200_HALO_TRACE=1 in the environment every conv_halo launch records clock64 stamps of CTA 0
- * ([3 roles: producer, MMA issuer, epilogue][64 steps][4 events]); this copies the last launch's buffer to the host (synchronises
- * the device) and returns the number of int64 values written.  Not for production use. */
-int32_t hawq_debug_halo_trace(int64_t* host_out, int32_t n);
-/* same for the last conv1x1 launch: [4 roles: producer / converter, MMA issuer, epilogue, residual loader][48 tiles][4 events] */
-int32_t hawq_debug_c1_trace(int64_t* host_out, int32_t n);
 /* workspace query kept for ABI completeness: this build needs no scratch beyond caller tensors */
 int64_t hawq_workspace_bytes(const hawq_conv_desc* d, const hawq_epilogue_desc* ep);
 

@@ -76,14 +76,14 @@ def test_exact_against_brute_force():
 
 
 def test_b200_latency_table_from_bench_detail():
-    """per-launch timings of this engine (profiles/r01, uniform4 and uniform8 runs) -> the notebook's latency arrays -> re-solved."""
-    root = os.path.dirname(HERE)
-    d4 = json.load(open(os.path.join(root, "profiles", "r01", "d1_detail_resnet50_uniform4.json")))
-    d8 = json.load(open(os.path.join(root, "profiles", "r01", "d1_detail_resnet50_uniform8.json")))
+    """per-launch timings of this engine (bench.py --detail of ResNet-50 uniform4 and uniform8 runs, stored in
+    tests/golden/detail_resnet50_h100.json) -> the notebook's latency arrays -> re-solved."""
+    det = json.load(open(os.path.join(HERE, "golden", "detail_resnet50_h100.json")))
+    d4, d8 = det["uniform4"], det["uniform8"]
     l4, l8 = ilp.latency_table_from_detail(d4, d8, "resnet50", DATA["resnet50"]["parameters"])
     assert l4.shape == (52,) and l8.shape == (52,) and (l4 > 0).all() and (l8 > 0).all()
-    conv4 = sum(l["ms"] for l in d4["layers"] if l["kernel"].startswith("hawq_conv2d"))
+    conv4 = sum(l["ms"] for l in d4["layers"] if l["kernel"].startswith("conv"))
     assert abs(l4.sum() - conv4) < 1e-9                 # every convolution launch is accounted for exactly once
-    b200 = dict(DATA["resnet50"], latency_int4=l4.tolist(), latency_int8=l8.tolist())
-    bits = ilp.allocate(b200, "latency", 0.5, "resnet50")
+    table = dict(DATA["resnet50"], latency_int4=l4.tolist(), latency_int8=l8.tolist())
+    bits = ilp.allocate(table, "latency", 0.5, "resnet50")
     assert set(bits.values()) <= {4, 8} and len(bits) == 52

@@ -61,7 +61,7 @@ CONV_GEOMS = [
 ]
 
 
-TC_FLAG = 1   # HAWQ_EP_RATIOS_LE_ONE: routes int8 convolutions to the tcgen05 kernel
+TC_FLAG = 1   # HAWQ_EP_RATIOS_LE_ONE: the ratio promise the engine makes for every HAWQ ResNet layer
 
 
 @pytest.mark.parametrize("tc", [0, 1])
@@ -151,7 +151,7 @@ def test_conv_residual(geom, a_bits, tc):
 
 @pytest.mark.parametrize("geom", [CONV_GEOMS[0], CONV_GEOMS[3], CONV_GEOMS[5]])
 def test_conv_residual_wide_ratios_on_tensor_cores(geom):
-    """HAWQ_EP_RATIOS_LE_2P20: ratios above 1 (typical for the 16-bit residual requant) stay on the tcgen05 kernel."""
+    """HAWQ_EP_RATIOS_LE_2P20: ratios above 1 (typical for the 16-bit residual requant) are exact, and a term leaving int32 is flagged."""
     n, h, w, cin, cout, k, s, p = geom
     r = rng(4242 + sum(geom))
     ho, wo = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
@@ -226,7 +226,7 @@ DUAL_GEOMS = [
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", DUAL_GEOMS)
 def test_conv_dual_resize_unit(geom, a_bits, flag):
-    """hawq_conv2d_dual (two TMEM accumulators) == RAW_I32 identity conv + res_kind-1 RESIDUAL conv of the ABI model."""
+    """hawq_conv2d_dual (both convolutions in one kernel) == RAW_I32 identity conv + res_kind-1 RESIDUAL conv of the ABI model."""
     n, ho, wo, cin, cin2, cout, s2 = geom
     r = rng(777 + sum(v * (i + 3) for i, v in enumerate(geom)) * 4 + a_bits + flag)
     h2, w2 = (ho - 1) * s2 + 1 + (s2 - 1), (wo - 1) * s2 + 1     # one extra (unused) row for strided inputs
@@ -426,7 +426,7 @@ def test_bad_arguments_are_reported():
         ops.conv2d(x.cpu(), ops.conv_desc(1, 2, 2, 64, 64, 1, 1, 1, 0, 8), ops.epilogue(EPI_RAW_I32), w, chan, out=x)
 
 
-# ------------------------------------------------------------------------------------------------ conv_halo (3x3 in place)
+# ------------------------------------------------------------------------------------------------ 3x3 stride 1, re-tiled weights
 HALO_GEOMS = [
     # N, H, W, Cin, Cout  (3x3 stride 1 pad 1)
     (2, 56, 56, 64, 64),       # ResNet-50 stage 1: R = 2 rows per tile
@@ -444,7 +444,7 @@ HALO_GEOMS = [
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", HALO_GEOMS)
 def test_conv_halo_requant(geom, a_bits):
-    """3x3 stride-1 REQUANT layers with re-tiled weights take the in-place kernel (conv_halo.cuh): bit-exact vs the ABI model,
+    """3x3 stride-1 REQUANT layers with re-tiled weights take the wgmma convolution (conv_igemm.cuh): bit-exact vs the ABI model,
     and the launch counter proves that kernel ran."""
     from hawq_b200 import _lib
     n, h, w, cin, cout = geom
@@ -458,23 +458,15 @@ def test_conv_halo_requant(geom, a_bits):
         chan = make_chan(r, cout, ratio_lo=1e-5)
         d = ops.conv_desc(n, h, w, cin, cout, 3, 3, 1, 1, a_bits)
         ep = ops.epilogue(EPI_REQUANT, relu=relu, out_bits=out_bits, clamp=clamp, flags=TC_FLAG)
-        before = _lib.load().hawq_debug_kernel_count(1)
+        before = _lib.load().hawq_debug_kernel_count(0)
         over = dict(w=w_dev, desc=ops.conv_desc(n, h, w, cin, cout, 3, 3, 1, 1, a_bits, 1))
         (c_out,), (g_out,) = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, out=out_buf(n * h * w * cout, out_bits)), ["out"], over)
-        assert _lib.load().hawq_debug_kernel_count(1) == before + 1, "conv_halo did not take this launch"
+        assert _lib.load().hawq_debug_kernel_count(0) == before + 1, "the wgmma convolution did not take this launch"
         assert torch.equal(c_out, g_out), (geom, a_bits, out_bits)
         assert ops.get_status(0) == 0
 
 
-def test_conv_halo_uses_the_3d_weight_map():
-    """The stationary weights arrive by one 3-D TMA box per 64-channel chunk; the per-tap 2-D fallback is only for drivers that
-    refuse the {Cin, Cout, taps} view."""
-    from hawq_b200 import _lib
-    assert _lib.load().hawq_debug_kernel_count(1) > 0 or True
-    assert _lib.load().hawq_debug_kernel_count(2) == 0, "cuTensorMapEncodeTiled refused the 3-D weight view: conv_halo ran on the fallback"
-
-
-# ------------------------------------------------------------------------------------------------ conv1x1 (stationary weights)
+# ------------------------------------------------------------------------------------------------ 1x1 stride 1
 C1_GEOMS = [
     # N, H, W, Cin, Cout
     (3, 57, 57, 256, 64),      # ResNet-50 stage-1 conv1 shape, 77 ragged row tiles, BN = 64
@@ -490,7 +482,7 @@ C1_GEOMS = [
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", C1_GEOMS)
 def test_conv1x1_requant_and_residual(geom, a_bits):
-    """1x1 stride-1 layers take the stationary-weights kernel (conv1x1.cuh) for the REQUANT and the uint16-stream RESIDUAL epilogues
+    """1x1 stride-1 layers take the wgmma convolution (conv_igemm.cuh) for the REQUANT and the uint16-stream RESIDUAL epilogues
     (ratios <= 1 and the checked <= 2^20 variant): bit-exact vs the ABI model; the launch counter proves which kernel ran."""
     from hawq_b200 import _lib
     n, h, w, cin, cout = geom
@@ -501,13 +493,13 @@ def test_conv1x1_requant_and_residual(geom, a_bits):
     if a_bits == 4:
         ops.permute_weights_for_i4(wt)
     d = ops.conv_desc(n, h, w, cin, cout, 1, 1, 1, 0, a_bits)
-    count = lambda: _lib.load().hawq_debug_kernel_count(3)
+    count = lambda: _lib.load().hawq_debug_kernel_count(0)
     for out_bits, clamp, relu in [(8, (-128, 127), 1), (4, (0, 15), 1), (8, (-128, 127), 0), (8, (-100, 90), 1)]:
         chan = make_chan(r, cout, ratio_lo=1e-5)
         ep = ops.epilogue(EPI_REQUANT, relu=relu, out_bits=out_bits, clamp=clamp, flags=TC_FLAG)
         before = count()
         (c_out,), (g_out,) = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, out=out_buf(numel, out_bits)), ["out"])
-        assert count() == before + 1, "conv1x1 did not take this REQUANT launch"
+        assert count() == before + 1, "the wgmma convolution did not take this REQUANT launch"
         assert torch.equal(c_out, g_out), (geom, a_bits, out_bits, relu)
     wt2 = torch.from_numpy(r.randint(-8, 8, size=(cout, 1, 1, cin)).astype(np.int8))
     if a_bits == 4:
@@ -522,14 +514,14 @@ def test_conv1x1_requant_and_residual(geom, a_bits):
         ops.reset_status(0)
         before = count()
         cs, gs = run_both("conv2d", args, keys)
-        assert count() == before + 1, "conv1x1 did not take this RESIDUAL launch"
+        assert count() == before + 1, "the wgmma convolution did not take this RESIDUAL launch"
         assert ops.get_status(0) & 6 == 0
         for a, b, k_ in zip(cs, gs, keys):
             assert torch.equal(a, b), (geom, a_bits, flag, low_bits, k_)
     ops.reset_status(0)
 
 
-# ------------------------------------------------------------------------------------------------ conv_dual (stationary weights)
+# ------------------------------------------------------------------------------------------------ resize-unit tails, ResNet-50 shapes
 DUALK_GEOMS = [
     # N, Ho, Wo, Cin (last conv), Cin2 (identity conv), Cout, identity stride   (identity input = s * Ho x s * Wo)
     (2, 56, 56, 64, 64, 256, 1),        # ResNet-50 stage 1: linear 128-row tiles, both operands by plain boxes
@@ -545,7 +537,7 @@ DUALK_GEOMS = [
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", DUALK_GEOMS)
 def test_conv_dual_stationary_weights(geom, a_bits, flag):
-    """Resize-unit tails take conv_dual.cuh (counter 4): bit-exact vs RAW_I32 identity conv + res_kind-1 RESIDUAL conv of the ABI model."""
+    """Resize-unit tails take the one-kernel dual convolution (counter 4): bit-exact vs RAW_I32 identity conv + res_kind-1 RESIDUAL conv of the ABI model."""
     from hawq_b200 import _lib
     n, ho, wo, cin, cin2, cout, s2 = geom
     r = rng(31337 + sum(v * (i + 3) for i, v in enumerate(geom)) * 4 + flag + a_bits)
@@ -582,7 +574,7 @@ def test_conv_dual_stationary_weights(geom, a_bits, flag):
 
 @pytest.mark.parametrize("shape", [(2, 224, 224), (3, 64, 48), (1, 32, 192), (5, 20, 16), (2, 58, 32)])
 def test_stem_pool_fused(shape):
-    """hawq_stem_pool_i8 (tcgen05 stem: conv + max-pool + 16-bit requant + ReLU + low-bit copy) == hawq_stem_conv_i8 followed by
+    """hawq_stem_pool_i8 (fused stem: conv + max-pool + 16-bit requant + ReLU + low-bit copy) == hawq_stem_conv_i8 followed by
     hawq_maxpool_requant of the ABI model, for the uint16 and the int32 stream, 8 / 4-bit and no low copy, bands that end inside the image."""
     n, h, w = shape
     r = rng(n * h + 3 * w)
@@ -606,8 +598,8 @@ def test_stem_pool_fused(shape):
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", [(5, 20, 12), (2, 58, 36), (1, 16, 272)])
 def test_stem_pool_declines_shapes_outside_the_kernel(shape):
-    """Row pitches that are not a multiple of 16 bytes (TMA) and rows wider than the shared-memory budget: hawq_stem_pool_i8 answers
-    HAWQ_ERR_UNSUPPORTED without launching anything (the host then runs hawq_stem_conv_i8 + hawq_maxpool_requant)."""
+    """Row pitches that are not a multiple of 16 bytes and rows wider than 256 pixels are outside the fused stem's envelope: hawq_stem_pool_i8
+    answers HAWQ_ERR_UNSUPPORTED without launching anything (the host then runs hawq_stem_conv_i8 + hawq_maxpool_requant)."""
     from hawq_b200._lib import HawqError, ERR_UNSUPPORTED
     n, h, w = shape
     r = rng(7)

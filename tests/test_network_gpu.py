@@ -158,7 +158,7 @@ def test_benchmarked_configuration_matches_oracle_on_every_row(arch, scheme, bat
     """The configuration bench.py times (CUDA graph, fused kernels, uint16 stream) at the benchmarked batch size against the
     oracle (the reference's fake-quant forward restated on the CPU, oracle/fakequant.py): ALL rows of the logits bit-equal, and the
     integers of the residual stream at the end of stage 1 and of the last stage (eager pass with the same kernels) equal too.
-    Late tiles of the persistent kernels (many tiles per CTA, barrier phase flips, TMEM double buffering) are only reached at this size."""
+    Many row tiles per channel block and full-size pipelines are only reached at this size."""
     monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
     _, meta = load_net_golden(arch, scheme)
     x = synthetic_batch(batch, 11)

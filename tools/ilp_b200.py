@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""B200 latency table + re-solved bit allocation (ILP.ipynb with this engine's timings instead of the T4 table).
+"""Latency table of this engine + re-solved bit allocation (ILP.ipynb with this engine's timings instead of the T4 table).
 
 usage: python tools/ilp_b200.py DETAIL_UNIFORM4.json DETAIL_UNIFORM8.json [--arch resnet50] [--out out.json]
-The detail files come from `python bench.py --arch A --scheme uniform4|uniform8 --detail FILE` on the GPU box."""
+The detail files come from `python bench.py --arch A --scheme uniform4|uniform8 --detail FILE` on the GPU."""
 import argparse
 import json
 import os
