@@ -132,6 +132,15 @@ int hawq_copy_status(hawq_handle* h, int32_t* dst, void* stream) {
   return HAWQ_OK;
 }
 
+// |acc| <= K * 128 * 128 (int8 activations) or K * 15 * 128 (unsigned 4-bit activations), int8 weights: a bias in
+// [bias_lo, bias_hi] keeps acc + bias inside int32, so the fast epilogues may add it without saturating
+static void set_bias_window(ConvParams& p, int a_bits) {
+  long long bound = (long long)p.K * (a_bits == 4 ? 15 * 128 : 128 * 128);
+  if (bound > 2147483648ll) bound = 2147483648ll;   // empty window: every bias takes the saturating epilogue
+  p.bias_lo = (int)(bound - 2147483648ll);
+  p.bias_hi = (int)(2147483647ll - bound);
+}
+
 static int check_me(uint32_t m, int e, const char* what) {
   if (e < 1 || e > 62 || m > 0x80000000u) return fail(HAWQ_ERR_BAD_ARG, "%s: dyadic pair out of range (m=%u e=%d)", what, m, e);
   return HAWQ_OK;
@@ -164,6 +173,7 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
   p.res_kind = ep->res_kind; p.res_bits = ep->res_bits; p.res_m = ep->res_m; p.res_e = ep->res_e;
   p.y_bits = ep->y_bits; p.low_bits = ep->low_bits; p.low_m = ep->low_m; p.low_e = ep->low_e;
   p.low_lo = ep->low_lo; p.low_hi = ep->low_hi; p.cout_store = ep->cout_store;
+  set_bias_window(p, d->a_bits);
   p.slow_scalar = 0;
   p.check_ovf = ep->mode == HAWQ_EPI_RESIDUAL && (ep->flags & (HAWQ_EP_RATIOS_LE_ONE | HAWQ_EP_RATIOS_LE_2P20)) != 0;
   if (ep->mode == HAWQ_EPI_RESIDUAL) {
@@ -261,6 +271,7 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
   p.mode = HAWQ_EPI_RESIDUAL; p.relu = 1; p.res_kind = 1; p.res_bits = 32; p.y_bits = 16; p.low_bits = ep->low_bits; p.low_m = ep->low_m;
   p.low_e = ep->low_e; p.low_lo = ep->low_lo; p.low_hi = ep->low_hi;
   p.check_ovf = 1;
+  set_bias_window(p, d->a_bits);   // main convolution only: the identity operand's bias is added with sat_add
   p.x2 = (const uint8_t*)x2; p.w2 = w2; p.H2 = d2->H; p.W2 = d2->W; p.stride2 = d2->stride; p.cin_chunks2 = d2->Cin / 64;
   p.x2_pix_bytes = d2->Cin * d2->a_bits / 8;
 

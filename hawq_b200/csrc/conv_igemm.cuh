@@ -47,6 +47,7 @@ struct ConvParams {
   int slow_scalar;   // host-checked: a scalar dyadic pair (res / low) has ratio > 1 -> generic 64-bit requant
   int wide_scalar_bad;   // host-checked: the scalar residual ratio exceeds 2^20 or the low-bit ratio exceeds 1 (no WIDE epilogue)
   int check_ovf;     // RESIDUAL under a HAWQ_EP_RATIOS_* promise: a requantised term leaving int32 raises HAWQ_FLAG_REQUANT_OVERFLOW
+  int bias_lo, bias_hi;   // host-computed from K and a_bits: a bias in [bias_lo, bias_hi] keeps acc + bias inside int32 (empty when bias_lo > bias_hi)
   // DUAL launches: the identity 1x1 convolution (res_chan holds its bias and per-channel identity ratio)
   const uint8_t* x2;
   const int8_t* w2;
@@ -85,8 +86,8 @@ __device__ __forceinline__ int swz(int row, int ch) {
   else return row * 32 + ((ch ^ ((row >> 2) & 1)) << 4);
 }
 
-// EPI selects the compile-time specialised fast epilogue (used when every dyadic ratio of the launch is <= 1, which the
-// kernel verifies): 0 = none (generic run-time epilogue only), 1 = REQUANT to 4/8 bits, 2 = RESIDUAL.
+// EPI selects the compile-time specialised fast epilogue (used when every dyadic ratio of the CTA is <= 1 and every bias keeps
+// acc + bias inside int32, which the kernel verifies): 0 = none (generic run-time epilogue only), 1 = REQUANT to 4/8 bits, 2 = RESIDUAL.
 constexpr int EPI_GENERIC = 0, EPI_FAST_LOW = 1, EPI_FAST_RES = 2;
 
 // geometry of one implicit GEMM of a launch (the main convolution, or the identity convolution of a DUAL launch)
@@ -126,11 +127,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
 
   int slow = p.slow_scalar;
   int wide_bad = p.wide_scalar_bad;   // some ratio > 2^20: the FP64 FMA is no longer exact for every int32 operand
+  int bias_wide = 0;                  // some acc + bias may leave int32: the folded (unsaturated) bias add would differ from sat_add
   if (tid < BN) {
     const hawq_chan c = p.chan[n0 + tid];
     sChan[tid] = c;
     sM[tid] = dyadic_to_double(c.m, c.e);
     sCb[tid] = 4503601774854144.0 - (double)c.bias;   // exact: folds the bias add into the int -> double conversion
+    bias_wide = c.bias < p.bias_lo || c.bias > p.bias_hi;
     slow |= !dyadic_is_fast(c.m, c.e);
     wide_bad |= !dyadic_is_wide(c.m, c.e);
     if (p.mode == HAWQ_EPI_RESIDUAL && p.res_kind == 1) {
@@ -145,6 +148,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   // RESIDUAL under a ratio promise with every ratio <= 2^20: the FP64 epilogue stays exact whenever a term fits int32, and every term
   // is range-checked (HAWQ_FLAG_REQUANT_OVERFLOW), so it replaces the generic epilogue (CTA-uniform)
   const bool use_wide = (__syncthreads_or(wide_bad) == 0) && use_slow && p.check_ovf && p.mode == HAWQ_EPI_RESIDUAL;
+  // the specialised epilogues add the bias without saturating (sCb); a CTA with a bias near the int32 limits takes the
+  // sat_add epilogue instead (CTA-uniform)
+  const bool bias_fold = __syncthreads_or(bias_wide) == 0;
 
   int32_t acc[NACC];
 
@@ -286,7 +292,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   bool fast_done = false;
 
   if constexpr (EPI == EPI_FAST_LOW) {
-    if (!use_slow) {
+    if (!use_slow && bias_fold) {
       fast_done = true;
       // clamp(RHE((acc + bias) * M)), ReLU folded into the lower clamp bound (RHE is monotone, RHE(0) = 0)
       const int lo = p.relu ? max(p.lo, 0) : p.lo, hi = p.hi;
@@ -311,7 +317,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   }
 
   if constexpr (EPI == EPI_FAST_RES) {
-    if (!use_slow || use_wide) {
+    if (bias_fold && (!use_slow || use_wide)) {
       fast_done = true;
       // t = fma(d, M, 1.5 * 2^52) with d * M exact inside the FMA: for |d * M| < 2^51 the low word of t is RHE(d * M); a term outside
       // int32 (which includes every |d * M| >= 2^51) is detected on t - 1.5 * 2^52 (exact in range, far out of range otherwise)

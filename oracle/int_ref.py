@@ -58,7 +58,7 @@ def requant(acc, m, e):
     """RHE(acc * m / 2^e); acc int64 [..., C], m/e scalars or [C]."""
     acc = np.asarray(acc, dtype=I64)
     m = np.asarray(m, dtype=I64)
-    assert np.abs(acc).max(initial=0) < 2 ** 31, "accumulator leaves int32"
+    assert acc.min(initial=0) >= -2 ** 31 and acc.max(initial=0) < 2 ** 31, "accumulator leaves int32"
     return rhe_shift(acc * m, e)
 
 

@@ -105,8 +105,9 @@ def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None,
             r = decode(res, ep.res_bits, ep.res_bits == 32).reshape(v.shape)
             m1, e1 = I64(ep.res_m), I64(ep.res_e)
         if ep.flags & 3:   # fast-path promise: a term leaving int32 raises HAWQ_FLAG_REQUANT_OVERFLOW (contents then unspecified)
-            if max(np.abs(ir.requant(r, m1, e1)).max(initial=0), np.abs(ir.requant(v, m, e)).max(initial=0)) >= 2 ** 31:
-                status["flags"] |= 4
+            for q in (ir.requant(r, m1, e1), ir.requant(v, m, e)):
+                if q.min(initial=0) < -2 ** 31 or q.max(initial=0) > 2 ** 31 - 1:
+                    status["flags"] |= 4
         y = sat32(rq(r, m1, e1) + rq(v, m, e))
         if ep.relu:
             y = np.maximum(y, 0)

@@ -81,14 +81,18 @@ def test_host_requant_exact_ties(lib, q, k, odd_shift):
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
-# The arithmetic of the fused epilogues (hawq_b200/csrc/common.cuh, conv_tc.cuh), modelled with exact rationals: one FP64 FMA with
-# the 1.5 * 2^52 constant rounds (v + bias) * m / 2^e once, to nearest-even, and the low mantissa word is the integer result.
+# The arithmetic of the fused epilogues (hawq_b200/csrc/common.cuh, conv_igemm.cuh), modelled with exact rationals: one FP64 FMA
+# with the 1.5 * 2^52 constant rounds (v + bias) * m / 2^e once, to nearest-even, and the low mantissa word is the integer result.
 # float(Fraction) is correctly rounded, so this checks the ALGORITHM (not the CUDA code, which the -m gpu tests cover).
 import struct  # noqa: E402
+
+from hypothesis import example  # noqa: E402
 
 MAGIC = 3 * 2 ** 51            # 1.5 * 2^52
 OFF_S = 2 ** 52 + 2 ** 31      # double({0x43300000, v ^ 0x80000000}) = 2^52 + 2^31 + v
 OFF_U = 2 ** 52                # double({0x43300000, u})              = 2^52 + u
+K_DEEP = 3 * 3 * 512           # deepest ResNet convolution (72 k-tiles)
+ACC_BOUND = {8: K_DEEP * 128 * 128, 4: K_DEEP * 15 * 128}   # |acc| for int8 / unsigned 4-bit activations, int8 weights
 
 
 def _lo_word(y):
@@ -97,11 +101,25 @@ def _lo_word(y):
     return lo - 2 ** 32 if lo >= 2 ** 31 else lo, bits >> 32
 
 
-def fast_signed(v, bias, m, e):
-    d = float(OFF_S + v)                                   # exact: < 2^53
-    cb = float(OFF_S - bias)                               # exact
-    dv = d - cb                                            # exact: v + bias
-    assert Fraction(dv) == v + bias
+def sat32(v):
+    return max(-2 ** 31, min(2 ** 31 - 1, v))
+
+
+def bias_window(acc_bound):
+    """set_bias_window (api.cu): the biases for which acc + bias stays inside int32 for every |acc| <= acc_bound."""
+    b = min(acc_bound, 2 ** 31)
+    return b - 2 ** 31, 2 ** 31 - 1 - b
+
+
+def fast_signed(v, bias, m, e, acc_bound=ACC_BOUND[8]):
+    lo, hi = bias_window(acc_bound)
+    if lo <= bias <= hi:                                   # bias folded into the int -> double conversion (sCb), not saturated
+        d = float(OFF_S + v)                               # exact: < 2^53
+        cb = float(OFF_S - bias)                           # exact
+        dv = d - cb                                        # exact: v + bias
+        assert Fraction(dv) == v + bias
+    else:                                                  # the CTA takes the sat_add epilogue
+        dv = float(sat32(v + bias))
     y = float(Fraction(dv) * Fraction(m, 2 ** e) + MAGIC)  # the FMA: one rounding
     return _lo_word(y)
 
@@ -114,11 +132,24 @@ def fast_unsigned_folded(u, m, e):
     return _lo_word(y)[0]
 
 
-@settings(max_examples=600, deadline=None)
-@given(st.integers(-2 ** 30, 2 ** 30), st.integers(-2 ** 29 + 1, 2 ** 29 - 1), st.integers(0, 2 ** 31), st.integers(31, 62))
-def test_fma_requant_is_exact_for_ratios_up_to_one(v, bias, m, e):
-    q, _ = fast_signed(v, bias, m, e)
-    assert q == rhe_exact(v + bias, m, e)
+M_5E8, E_5E8 = ir.dyadic(5e-8)   # a near-dead channel: tiny ratio, bias at the int32 limit
+
+
+@settings(max_examples=1000, deadline=None)
+@given(st.sampled_from([8, 4]), st.integers(-ACC_BOUND[8], ACC_BOUND[8]), st.integers(-2 ** 31, 2 ** 31 - 1), st.integers(0, 2 ** 31),
+       st.integers(31, 62))
+@example(8, ACC_BOUND[8], 2 ** 31 - 1, 2 ** 31, 31)
+@example(8, -ACC_BOUND[8], -2 ** 31, 2 ** 31, 31)
+@example(4, ACC_BOUND[8], 2 ** 31 - 1, 2 ** 31, 31)
+@example(8, 5_000_000, 2 ** 31 - 1, M_5E8, E_5E8)
+@example(8, -5_000_000, -2 ** 31, M_5E8, E_5E8)
+@example(8, 75_000_000, 2 ** 31 - 1000, 2 ** 31, 31)
+def test_fma_requant_is_exact_for_ratios_up_to_one(a_bits, v, bias, m, e):
+    """acc up to the K = 4608 bound of either activation width, any int32 bias: the epilogue equals RHE(sat32(acc + bias) * ratio)."""
+    if a_bits == 4:
+        v = v * 15 // 128                                  # |acc| <= K * 15 * 128
+    q, _ = fast_signed(v, bias, m, e, ACC_BOUND[a_bits])
+    assert q == rhe_exact(sat32(v + bias), m, e)
 
 
 @settings(max_examples=600, deadline=None)
@@ -131,7 +162,7 @@ def test_fma_requant_wide_ratios_with_overflow_check(v, bias, m, e):
     fl = math.floor(exact)
     rem = exact - fl
     r = fl + (1 if rem > Fraction(1, 2) or (rem == Fraction(1, 2) and fl % 2 == 1) else 0)   # unsaturated RHE
-    valid = ((hi + ((q >> 31) & 1)) ^ 0x43380000) == 0                                       # the check in conv_tc.cuh (WIDE)
+    valid = ((hi + ((q >> 31) & 1)) ^ 0x43380000) == 0          # bit-pattern form of the WIDE check in conv_igemm.cuh (t - 1.5 * 2^52 in int32)
     assert valid == (-2 ** 31 <= r < 2 ** 31)
     if valid:
         assert q == r

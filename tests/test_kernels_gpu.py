@@ -39,26 +39,42 @@ def out_buf(numel, bits):
 
 
 def run_both(fn_name, cpu_args, out_keys, gpu_overrides=None):
-    """cpu_args: dict of kwargs with CPU tensors; out_keys: names of output tensors.  Returns (cpu_outs, gpu_outs)."""
+    """cpu_args: dict of kwargs with CPU tensors; out_keys: names of output tensors.  Returns (cpu_outs, gpu_outs).
+    Both status words start at 0, and the library's must equal the model's after the call."""
     gpu_args = {k: (v.to(DEV) if torch.is_tensor(v) else v) for k, v in cpu_args.items()}
     gpu_args.update(gpu_overrides or {})
+    ops.reset_status(0)
+    am.status["flags"] = 0
     getattr(am, fn_name)(**cpu_args)
     getattr(ops, fn_name)(**gpu_args)
     torch.cuda.synchronize()
+    assert ops.get_status(0) == am.status["flags"], (fn_name, ops.get_status(0), am.status["flags"])
     return [cpu_args[k] for k in out_keys], [gpu_args[k].cpu() for k in out_keys]
 
 
 CONV_GEOMS = [
-    # N, H, W, Cin, Cout, k, stride, pad
-    (2, 8, 8, 64, 64, 1, 1, 0),
-    (3, 7, 7, 64, 128, 3, 1, 1),       # M = 147: ragged last tile
-    (2, 14, 14, 128, 64, 3, 2, 1),
-    (2, 9, 9, 256, 256, 1, 2, 0),
-    (1, 20, 12, 64, 192, 3, 1, 1),     # Cout = 192 -> BN = 64 path with 3 column tiles
-    (5, 6, 6, 128, 128, 3, 1, 1),
-    (3, 7, 7, 128, 128, 1, 1, 0),      # 1x1 stride 1, M = 147: TMA-fed activations with a ragged (zero-filled) last tile
-    (2, 5, 5, 192, 256, 1, 1, 0),      # M = 50 < one tile, K = 3 k-tiles
+    # N, H, W, Cin, Cout, kh, kw, stride, pad
+    (2, 8, 8, 64, 64, 1, 1, 1, 0),
+    (3, 7, 7, 64, 128, 3, 3, 1, 1),       # M = 147: ragged last tile
+    (2, 14, 14, 128, 64, 3, 3, 2, 1),
+    (2, 9, 9, 256, 256, 1, 1, 2, 0),
+    (1, 20, 12, 64, 192, 3, 3, 1, 1),     # Cout = 192 -> BN = 64 path with 3 column tiles
+    (5, 6, 6, 128, 128, 3, 3, 1, 1),
+    (3, 7, 7, 128, 128, 1, 1, 1, 0),      # 1x1 stride 1, M = 147: ragged (zero-filled) last tile
+    (2, 5, 5, 192, 256, 1, 1, 1, 0),      # M = 50 < one tile, K = 3 k-tiles
+    (2, 7, 7, 512, 128, 3, 3, 1, 1),      # K = 4608, 72 k-tiles: the deepest ResNet layer
+    (2, 9, 9, 64, 64, 5, 5, 1, 2),
+    (2, 15, 15, 64, 128, 7, 7, 2, 3),
+    (2, 8, 8, 64, 128, 1, 3, 1, 0),
+    (2, 8, 8, 64, 64, 3, 1, 1, 0),
+    (2, 7, 7, 64, 64, 1, 1, 1, 1),        # 1x1 with padding: the border ring of outputs sees only zeros
+    (2, 11, 11, 64, 128, 3, 3, 3, 2),
+    (3, 2, 3, 64, 64, 5, 5, 1, 2),        # input smaller than the kernel
 ]
+
+
+def out_hw(h, w, kh, kw, s, p):
+    return (h + 2 * p - kh) // s + 1, (w + 2 * p - kw) // s + 1
 
 
 TC_FLAG = 1   # HAWQ_EP_RATIOS_LE_ONE: the ratio promise the engine makes for every HAWQ ResNet layer
@@ -68,20 +84,20 @@ TC_FLAG = 1   # HAWQ_EP_RATIOS_LE_ONE: the ratio promise the engine makes for ev
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", CONV_GEOMS)
 def test_conv_requant(geom, a_bits, tc):
-    n, h, w, cin, cout, k, s, p = geom
+    n, h, w, cin, cout, kh, kw, s, p = geom
     r = rng(sum(v * (i + 3) for i, v in enumerate(geom)) * 8 + a_bits)
-    ho, wo = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    ho, wo = out_hw(h, w, kh, kw, s, p)
     x = rand_act(r, n * h * w * cin, a_bits)
-    wt = torch.from_numpy(r.randint(-128 if a_bits == 8 else -8, 128 if a_bits == 8 else 8, size=(cout, k, k, cin)).astype(np.int8))
+    wt = torch.from_numpy(r.randint(-128 if a_bits == 8 else -8, 128 if a_bits == 8 else 8, size=(cout, kh, kw, cin)).astype(np.int8))
     if a_bits == 4:
         ops.permute_weights_for_i4(wt)
     for out_bits, clamp, relu in [(8, (-128, 127), 1), (4, (0, 15), 1), (16, (-32768, 32767), 0), (32, (-2 ** 31, 2 ** 31 - 1), 0)]:
         chan = make_chan(r, cout, ratio_lo=1e-5 if out_bits <= 8 else 1e-3)
-        d = ops.conv_desc(n, h, w, cin, cout, k, k, s, p, a_bits)
+        d = ops.conv_desc(n, h, w, cin, cout, kh, kw, s, p, a_bits)
         ep = ops.epilogue(EPI_REQUANT, relu=relu, out_bits=out_bits, clamp=clamp, flags=TC_FLAG * tc)
         over = None
         if tc and DEV != "cpu" and (n + h) % 2 == 0:   # half of the geometries: weights re-tiled for linear bulk loads (w_layout = 1)
-            over = dict(w=ops.upload_weights(wt, DEV), desc=ops.conv_desc(n, h, w, cin, cout, k, k, s, p, a_bits, 1))
+            over = dict(w=ops.upload_weights(wt, DEV), desc=ops.conv_desc(n, h, w, cin, cout, kh, kw, s, p, a_bits, 1))
         (c_out,), (g_out,) = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, out=out_buf(n * ho * wo * cout, out_bits)), ["out"], over)
         assert torch.equal(c_out, g_out), (geom, a_bits, out_bits, tc)
 
@@ -123,16 +139,16 @@ def test_conv_requant_ties_and_generic_path(ratio_kind):
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", CONV_GEOMS[:4] + CONV_GEOMS[6:])
 def test_conv_residual(geom, a_bits, tc):
-    n, h, w, cin, cout, k, s, p = geom
+    n, h, w, cin, cout, kh, kw, s, p = geom
     r = rng(sum(v * (i + 5) for i, v in enumerate(geom)) * 8 + a_bits + 1)
-    ho, wo = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    ho, wo = out_hw(h, w, kh, kw, s, p)
     numel = n * ho * wo * cout
     x = rand_act(r, n * h * w * cin, a_bits)
-    wt = torch.from_numpy(r.randint(-8, 8, size=(cout, k, k, cin)).astype(np.int8))
+    wt = torch.from_numpy(r.randint(-8, 8, size=(cout, kh, kw, cin)).astype(np.int8))
     if a_bits == 4:
         ops.permute_weights_for_i4(wt)
     chan = make_chan(r, cout, ratio_lo=1e-2, ratio_hi=0.9)
-    d = ops.conv_desc(n, h, w, cin, cout, k, k, s, p, a_bits)
+    d = ops.conv_desc(n, h, w, cin, cout, kh, kw, s, p, a_bits)
     low_me = dyadic(0.004)
     for res_kind, res_bits, y_bits, low_bits, relu in [(0, 32, 32, 8, 1), (0, 16, 16, 4, 1), (1, 32, 32, 4, 1),
                                                        (0, 32, 32, 0, 0), (1, 32, 0, 8, 1), (0, 16, 16, 8, 1)]:
@@ -152,14 +168,14 @@ def test_conv_residual(geom, a_bits, tc):
 @pytest.mark.parametrize("geom", [CONV_GEOMS[0], CONV_GEOMS[3], CONV_GEOMS[5]])
 def test_conv_residual_wide_ratios_on_tensor_cores(geom):
     """HAWQ_EP_RATIOS_LE_2P20: ratios above 1 (typical for the 16-bit residual requant) are exact, and a term leaving int32 is flagged."""
-    n, h, w, cin, cout, k, s, p = geom
+    n, h, w, cin, cout, kh, kw, s, p = geom
     r = rng(4242 + sum(geom))
-    ho, wo = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    ho, wo = out_hw(h, w, kh, kw, s, p)
     numel = n * ho * wo * cout
     x = rand_act(r, n * h * w * cin, 8)
-    wt = torch.from_numpy(r.randint(-8, 8, size=(cout, k, k, cin)).astype(np.int8))
+    wt = torch.from_numpy(r.randint(-8, 8, size=(cout, kh, kw, cin)).astype(np.int8))
     chan = make_chan(r, cout, bias_mag=2000, ratio_lo=0.2, ratio_hi=40.0)
-    d = ops.conv_desc(n, h, w, cin, cout, k, k, s, p, 8)
+    d = ops.conv_desc(n, h, w, cin, cout, kh, kw, s, p, 8)
     for res_kind, res_bits, y_bits, low_bits in [(0, 16, 16, 8), (0, 32, 32, 4), (1, 32, 16, 8)]:
         res = rand_act(r, numel, res_bits if res_kind == 0 else 32)
         if res_bits == 16 and res_kind == 0:
@@ -167,10 +183,8 @@ def test_conv_residual_wide_ratios_on_tensor_cores(geom):
         res_chan = make_chan(r, cout, ratio_lo=0.5, ratio_hi=3.0) if res_kind == 1 else None
         ep = ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=res_kind, res_bits=res_bits, res_me=dyadic(1.37), y_bits=y_bits,
                           low_bits=low_bits, low_me=dyadic(0.0004), low_clamp=(0, 15) if low_bits == 4 else (-128, 127), flags=2)
-        ops.reset_status(0)
         cs, gs = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, res=res, res_chan=res_chan, out=out_buf(numel, y_bits),
                                          out_low=out_buf(numel, low_bits)), ["out", "out_low"])
-        assert ops.get_status(0) & 6 == 0
         for a, b in zip(cs, gs):
             assert torch.equal(a, b), (geom, res_kind, res_bits, y_bits, low_bits)
     # a term that leaves int32 on the fast path must raise HAWQ_FLAG_REQUANT_OVERFLOW (the generic kernel would saturate)
@@ -184,11 +198,11 @@ def test_conv_residual_wide_ratios_on_tensor_cores(geom):
 
 WS_GEOMS = [
     # N, H, W, Cin, Cout, k, stride, pad : REQUANT with re-tiled weights (w_layout 1), more tiles than SMs
-    (7, 56, 56, 64, 64, 3, 1, 1),      # patch mode, 172 tiles: several tiles per CTA, one channel block
+    (7, 56, 56, 64, 64, 3, 1, 1),      # 172 row tiles, one channel block
     (4, 49, 49, 128, 128, 3, 1, 1),    # K = 1152, 152 tiles
-    (3, 57, 57, 256, 256, 1, 1, 0),    # 1x1 stride 1 (TMA-fed int8 / gather 4-bit), 154 tiles, 2 channel blocks
-    (2, 31, 31, 128, 128, 1, 2, 0),    # strided 1x1: gather mode
-    (2, 30, 30, 64, 192, 3, 2, 1),     # strided 3x3: gather mode, 3 narrow channel blocks
+    (3, 57, 57, 256, 256, 1, 1, 0),    # 1x1 stride 1, 154 tiles, 2 channel blocks
+    (2, 31, 31, 128, 128, 1, 2, 0),    # strided 1x1
+    (2, 30, 30, 64, 192, 3, 2, 1),     # strided 3x3, 3 narrow channel blocks
     (1, 9, 9, 64, 64, 1, 1, 0),        # single k-tile, single ragged tile
 ]
 
@@ -251,12 +265,9 @@ def test_conv_dual_resize_unit(geom, a_bits, flag):
         args = dict(x=x, desc=d, ep=ep, w=wt, chan=chan, desc2=d2, x2=x2, w2=wt2, chan2=chan2, out=out_buf(numel, 16),
                     out_low=out_buf(numel, low_bits) if low_bits else None)
         keys = ["out"] + (["out_low"] if low_bits else [])
-        ops.reset_status(0)
         cs, gs = run_both("conv2d_dual", args, keys, gpu_overrides=dict(w=wg, w2=wg2))
-        assert ops.get_status(0) & 6 == 0
         for a, b, k_ in zip(cs, gs, keys):
             assert torch.equal(a, b), (geom, a_bits, flag, low_bits, k_)
-    ops.reset_status(0)
 
 
 def test_conv_dual_rejects_unsupported():
@@ -511,25 +522,22 @@ def test_conv1x1_requant_and_residual(geom, a_bits):
                           low_me=dyadic(0.004 if flag == 1 else 0.0004), low_clamp=(0, 15) if low_bits == 4 else (-128, 127), flags=flag)
         args = dict(x=x, desc=d, ep=ep, w=wt2, chan=chan, res=res, out=out_buf(numel, 16), out_low=out_buf(numel, low_bits) if low_bits else None)
         keys = [k_ for k_ in ("out", "out_low") if args[k_] is not None]
-        ops.reset_status(0)
         before = count()
         cs, gs = run_both("conv2d", args, keys)
         assert count() == before + 1, "the wgmma convolution did not take this RESIDUAL launch"
-        assert ops.get_status(0) & 6 == 0
         for a, b, k_ in zip(cs, gs, keys):
             assert torch.equal(a, b), (geom, a_bits, flag, low_bits, k_)
-    ops.reset_status(0)
 
 
 # ------------------------------------------------------------------------------------------------ resize-unit tails, ResNet-50 shapes
 DUALK_GEOMS = [
     # N, Ho, Wo, Cin (last conv), Cin2 (identity conv), Cout, identity stride   (identity input = s * Ho x s * Wo)
-    (2, 56, 56, 64, 64, 256, 1),        # ResNet-50 stage 1: linear 128-row tiles, both operands by plain boxes
-    (3, 28, 28, 128, 256, 512, 2),      # stage 2: tiles of 4 output rows (112), identity rows by the strided 5-D box
-    (2, 14, 14, 256, 512, 1024, 2),     # stage 3: 7 rows (98)
-    (5, 7, 7, 512, 1024, 2048, 2),      # stage 4: two images per tile (98), odd batch -> half-empty last tile; BN = 64
-    (2, 12, 12, 64, 128, 192, 2),       # Cout = 192 -> BN = 64, tiles of 6 rows (72)
-    (9, 4, 4, 64, 64, 128, 2),          # eight images per tile
+    (2, 56, 56, 64, 64, 256, 1),        # ResNet-50 stage 1: 49 row tiles of 128
+    (3, 28, 28, 128, 256, 512, 2),      # stage 2: strided identity input, ragged last row tile
+    (2, 14, 14, 256, 512, 1024, 2),     # stage 3
+    (5, 7, 7, 512, 1024, 2048, 2),      # stage 4: M = 245, half-empty last row tile
+    (2, 12, 12, 64, 128, 192, 2),       # Cout = 192 -> BN = 64
+    (9, 4, 4, 64, 64, 128, 2),          # eight images per row tile
 ]
 
 
@@ -537,7 +545,8 @@ DUALK_GEOMS = [
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", DUALK_GEOMS)
 def test_conv_dual_stationary_weights(geom, a_bits, flag):
-    """Resize-unit tails take the one-kernel dual convolution (counter 4): bit-exact vs RAW_I32 identity conv + res_kind-1 RESIDUAL conv of the ABI model."""
+    """Resize-unit tails take the one-kernel dual convolution (hawq_debug_kernel_count family 4, hawq_conv2d_dual): bit-exact vs
+    RAW_I32 identity conv + res_kind-1 RESIDUAL conv of the ABI model."""
     from hawq_b200 import _lib
     n, ho, wo, cin, cin2, cout, s2 = geom
     r = rng(31337 + sum(v * (i + 3) for i, v in enumerate(geom)) * 4 + flag + a_bits)
@@ -562,14 +571,11 @@ def test_conv_dual_stationary_weights(geom, a_bits, flag):
         args = dict(x=x, desc=d, ep=ep, w=wt, chan=chan, desc2=d2, x2=x2, w2=wt2, chan2=chan2, out=out_buf(numel, 16),
                     out_low=out_buf(numel, low_bits) if low_bits else None)
         keys = ["out"] + (["out_low"] if low_bits else [])
-        ops.reset_status(0)
         before = _lib.load().hawq_debug_kernel_count(4)
         cs, gs = run_both("conv2d_dual", args, keys, gpu_overrides=dict(w=wg, w2=wg2))
         assert _lib.load().hawq_debug_kernel_count(4) == before + 1, "conv_dual did not take this launch"
-        assert ops.get_status(0) & 6 == 0
         for a, b, k_ in zip(cs, gs, keys):
             assert torch.equal(a, b), (geom, a_bits, flag, low_bits, k_)
-    ops.reset_status(0)
 
 
 @pytest.mark.parametrize("shape", [(2, 224, 224), (3, 64, 48), (1, 32, 192), (5, 20, 16), (2, 58, 32)])
@@ -613,3 +619,294 @@ def test_stem_pool_declines_shapes_outside_the_kernel(shape):
         ops.stem_pool(x, wt, chan, (-32768, 32767), n, h, w, 16, y, 0, (0, 1), (0, 0), None)
     assert err.value.code == ERR_UNSUPPORTED
     assert int(y.abs().max()) == 0
+
+
+# ------------------------------------------------------------------------------------------------ int32 and ratio boundaries
+# The specialised epilogues of conv_igemm.cuh fold the bias into the int -> double conversion and run one FP64 FMA per term; a CTA
+# leaves them for the saturating or the exact 64-bit epilogue when a bias or a ratio is outside their range.  These tests put
+# accumulators, biases and ratios on those limits, side by side with ordinary channels in neighbouring column blocks, and demand
+# whole outputs and the status word equal to the ABI model.
+I32_MIN, I32_MAX = -2 ** 31, 2 ** 31 - 1
+RATIO_ONE = (2 ** 31, 31)           # exactly 1 in the specialised-epilogue form (dyadic(1.0) is (2^30, 30))
+WIDE_RATIOS = [dyadic(1.0), dyadic(1 + 2 ** -20), (2 ** 31, 11), dyadic(3.0), dyadic(1000.0)]   # (1, 2^20], 2^20 exactly
+GENERIC_RATIOS = [(2 ** 30 + 1, 10), (2 ** 31, 10), (0, 31), RATIO_ONE]                         # above 2^20, m = 0, 1
+
+
+def bias_window(k, a_bits):
+    """the biases for which acc + bias cannot leave int32: |acc| <= K * 128 * 128 (int8) or K * 15 * 128 (unsigned 4-bit)"""
+    b = min(k * (15 if a_bits == 4 else 128) * 128, 2 ** 31)
+    return b - 2 ** 31, 2 ** 31 - 1 - b
+
+
+def edge_biases(k, a_bits):
+    lo, hi = bias_window(k, a_bits)
+    return [I32_MIN, I32_MIN + 1, I32_MAX, lo - 1, lo, hi, hi + 1, 0]
+
+
+def extreme_act(r, n, pix, c, a_bits):
+    """image i % 3 == 0: every value -128 (4-bit: 15); 1: 127 (4-bit: 0); 2: random.  With a constant weight row, the outputs of
+    the first two images whose window lies inside the image reach acc = K * x * w exactly (K * 128 * 128 for x = w = -128)."""
+    consts = (-128, 127) if a_bits == 8 else (15, 0)
+    v = r.randint(-128, 128, size=(n, pix * c)) if a_bits == 8 else r.randint(0, 16, size=(n, pix * c))
+    for i in range(n):
+        if i % 3 < 2:
+            v[i] = consts[i % 3]
+    v = v.reshape(-1)
+    return torch.from_numpy(am.pack_i4(v)) if a_bits == 4 else torch.from_numpy(v.astype(np.int8))
+
+
+def boundary_weights_chan(r, cout, bn, kh, kw, cin, a_bits):
+    """Column block b (BN channels) by b % 4:
+      0: random weights, |bias| <= 2^16, ratios <= 1 (0.5 and 0.25 give round-half-even ties): the specialised epilogue;
+      1: bias edges (int32 limits, both sides of the bias window, 0) on constant weight rows -128 / 127 / -127 and random rows,
+         ratios <= 1 (1 exactly, 5e-8, m = 0, log-uniform down to 1e-9);
+      2: as 1, plus zero-weight channels with a small bias and a ratio in (1, 2^20] (the checked wide epilogue's range);
+      3: as 0, plus zero-weight channels with a small bias and a ratio above 2^20, m = 0 or exactly 1 (the exact 64-bit epilogue).
+    Zero-weight channels keep |bias| <= 1000, so that no term leaves int32 at ratios up to 2^21."""
+    k = kh * kw * cin
+    edges = edge_biases(k, a_bits)
+    w = r.randint(-128, 128, size=(cout, kh, kw, cin))
+    bias, me = [], []
+    for c in range(cout):
+        kind, j = (c // bn) % 4, c % bn
+        if kind in (0, 3):
+            b = int(r.randint(-2 ** 16, 2 ** 16))
+            ratio = [0.5, 0.25][j % 2] if j % 4 < 2 else float(np.exp(r.uniform(np.log(1e-5), 0.0)))
+            mc = dyadic(ratio)
+        else:
+            b = edges[j % 8]
+            row = (-128, 127, -127, None)[(j // 8) % 4]
+            if row is not None:
+                w[c] = row
+            mc = [RATIO_ONE, dyadic(5e-8), (0, 31), None, None][j % 5] or dyadic(float(np.exp(r.uniform(np.log(1e-9), 0.0))))
+        if (kind == 2 and j % 16 == 15) or (kind == 3 and j % 8 == 7):
+            ratios = WIDE_RATIOS if kind == 2 else GENERIC_RATIOS
+            w[c] = 0
+            b = int(r.randint(-1000, 1001))
+            mc = ratios[(j // 16 if kind == 2 else j // 8) % len(ratios)]
+        bias.append(b)
+        me.append(mc)
+    wt = torch.from_numpy(w.astype(np.int8))
+    if a_bits == 4:
+        ops.permute_weights_for_i4(wt)
+    return wt, ops.make_chan(bias, [m for m, _ in me], [e for _, e in me])
+
+
+def res_chan_with_ties(r, cout):
+    """per-channel ratios of a res_kind 1 operand: 0.5 and 0.25 (ties on every odd operand, negative ones included), else <= 1"""
+    me = [dyadic([0.5, 0.25][c % 2] if c % 4 < 2 else float(np.exp(r.uniform(np.log(1e-3), 0.0)))) for c in range(cout)]
+    return ops.make_chan([0] * cout, [m for m, _ in me], [e for _, e in me])
+
+
+BOUNDARY_GEOMS = [
+    # N, H, W, Cin, Cout, kh, kw, stride, pad: ragged last row tile in each
+    (3, 6, 6, 64, 320, 3, 3, 1, 1),       # BN = 64: five column blocks, M = 108
+    (3, 5, 5, 512, 512, 3, 3, 1, 1),      # BN = 128, K = 4608 (72 k-tiles), M = 75
+    (3, 9, 9, 128, 512, 1, 1, 1, 0),      # 1x1, M = 243: two row tiles
+]
+REQUANT_CASES = [(out_bits, clamp, relu) for out_bits, clamp in [(4, (0, 15)), (8, (-128, 127)), (16, (-32768, 32767)), (32, (I32_MIN, I32_MAX))]
+                 for relu in (0, 1)]
+RESIDUAL_CASES = [  # res_kind, res_bits, y_bits, low_bits, relu
+    (0, 16, 16, 8, 1), (0, 32, 32, 4, 1), (0, 32, 32, 0, 0), (0, 16, 0, 4, 1), (1, 32, 16, 4, 1), (1, 32, 0, 8, 1), (1, 32, 32, 0, 0)]
+
+
+@pytest.mark.parametrize("flags", [0, 1, 2])
+@pytest.mark.parametrize("a_bits", [8, 4])
+@pytest.mark.parametrize("geom", BOUNDARY_GEOMS)
+def test_conv_epilogue_boundaries(geom, a_bits, flags):
+    """Every conv2d epilogue at saturating biases and ratio edges, under each ratio promise (flags 1 with ratios above 1 is a broken
+    promise: the output must still be exact)."""
+    n, h, w, cin, cout, kh, kw, s, p = geom
+    r = rng(2024 + sum(v * (i + 3) for i, v in enumerate(geom)) * 8 + a_bits + 97 * flags)
+    ho, wo = out_hw(h, w, kh, kw, s, p)
+    numel = n * ho * wo * cout
+    x = extreme_act(r, n, h * w, cin, a_bits)
+    wt, chan = boundary_weights_chan(r, cout, 128 if cout % 128 == 0 else 64, kh, kw, cin, a_bits)
+    d = ops.conv_desc(n, h, w, cin, cout, kh, kw, s, p, a_bits)
+    failed = []   # every epilogue is checked; the assertion at the end names all that differ
+
+    def check(ep, what, **bufs):
+        keys = [k_ for k_ in ("out", "out_low") if bufs.get(k_) is not None]
+        try:
+            cs, gs = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, **bufs), keys)
+        except AssertionError as status_mismatch:
+            failed.append((what, "status", str(status_mismatch)))
+            return
+        for a, b, k_ in zip(cs, gs, keys):
+            if not torch.equal(a, b):
+                failed.append((what, k_, int((a != b).sum())))
+
+    for out_bits, clamp, relu in REQUANT_CASES:
+        check(ops.epilogue(EPI_REQUANT, relu=relu, out_bits=out_bits, clamp=clamp, flags=flags), ("requant", out_bits, relu),
+              out=out_buf(numel, out_bits))
+    res_chan = res_chan_with_ties(r, cout)
+    for res_kind, res_bits, y_bits, low_bits, relu in RESIDUAL_CASES:
+        for res_ratio in (0.37, 1.37):
+            if res_bits == 16:
+                res = torch.from_numpy(r.randint(0, 65536, size=numel).astype(np.uint16).view(np.int16))
+            elif res_kind == 1 or res_ratio < 1:   # full int32 range: every term stays inside int32 at ratios <= 1
+                res = torch.from_numpy(r.randint(I32_MIN, I32_MAX, size=numel, dtype=np.int64).astype(np.int32))
+                res[:cout] = I32_MIN
+                res[cout:2 * cout] = I32_MAX
+            else:
+                res = rand_act(r, numel, 32)
+            ep = ops.epilogue(EPI_RESIDUAL, relu=relu, res_kind=res_kind, res_bits=res_bits, res_me=dyadic(res_ratio), y_bits=y_bits,
+                              low_bits=low_bits, low_me=dyadic(0.004), low_clamp=(0, 15) if low_bits == 4 else (-128, 127), flags=flags)
+            check(ep, ("residual", res_kind, res_bits, y_bits, low_bits, res_ratio), res=res, res_chan=res_chan if res_kind else None,
+                  out=out_buf(numel, y_bits) if y_bits else None, out_low=out_buf(numel, low_bits) if low_bits else None)
+    check(ops.epilogue(EPI_RAW_I32, flags=flags), "raw", out=out_buf(numel, 32))
+    assert not failed, (geom, a_bits, flags, failed)
+
+
+@pytest.mark.parametrize("flag", [1, 2])
+@pytest.mark.parametrize("a_bits", [8, 4])
+@pytest.mark.parametrize("cout", [320, 512])
+def test_conv_dual_boundaries(cout, a_bits, flag):
+    """hawq_conv2d_dual with saturating biases on both convolutions, identity ratios 0.5 / 0.25 (ties on negative operands) and the
+    ratio edges of boundary_weights_chan on the main convolution."""
+    n, ho, wo, cin, cin2, s2 = 3, 7, 7, 128, 64, 2                  # M = 147: ragged last row tile
+    r = rng(555 + cout + 7 * a_bits + flag)
+    h2, w2 = ho * s2, wo * s2
+    numel = n * ho * wo * cout
+    bn = 128 if cout % 128 == 0 else 64
+    x = extreme_act(r, n, ho * wo, cin, a_bits)
+    x2 = extreme_act(r, n, h2 * w2, cin2, a_bits)
+    wt, chan = boundary_weights_chan(r, cout, bn, 1, 1, cin, a_bits)
+    wt2, _ = boundary_weights_chan(r, cout, bn, 1, 1, cin2, a_bits)
+    edges = edge_biases(cin2, a_bits)
+    ties = res_chan_with_ties(r, cout)
+    chan2 = ties.clone()
+    chan2[:, 0] = torch.tensor([edges[c % 8] if (c // bn) % 2 else int(r.randint(-3000, 3001)) for c in range(cout)], dtype=torch.int32)
+    d = ops.conv_desc(n, ho, wo, cin, cout, 1, 1, 1, 0, a_bits, 1)
+    d2 = ops.conv_desc(n, h2, w2, cin2, cout, 1, 1, s2, 0, a_bits, 1)
+    wg, wg2 = ops.upload_weights(wt, DEV), ops.upload_weights(wt2, DEV)
+    for low_bits in (8, 4, 0):
+        ep = ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=1, res_bits=32, y_bits=16, low_bits=low_bits, low_me=dyadic(0.003),
+                          low_clamp=(0, 15) if low_bits == 4 else (-128, 127), flags=flag)
+        args = dict(x=x, desc=d, ep=ep, w=wt, chan=chan, desc2=d2, x2=x2, w2=wt2, chan2=chan2, out=out_buf(numel, 16),
+                    out_low=out_buf(numel, low_bits) if low_bits else None)
+        keys = ["out"] + (["out_low"] if low_bits else [])
+        cs, gs = run_both("conv2d_dual", args, keys, gpu_overrides=dict(w=wg, w2=wg2))
+        for a, b, k_ in zip(cs, gs, keys):
+            assert torch.equal(a, b), (cout, a_bits, flag, low_bits, k_, int((a != b).sum()))
+
+
+@pytest.mark.parametrize("a_bits", [8, 4])
+def test_rows_past_m_raise_no_flag(a_bits):
+    """Rows of a ragged tile past M are zero-filled, so there acc = 0 and v = bias.  With acc = -bias on every real row and a
+    ratio of 2^17, a zero-filled row would leave int32 (HAWQ_FLAG_REQUANT_OVERFLOW) and, for int8 inputs, exceed the uint16
+    stream (HAWQ_FLAG_RESIDUAL_OVERFLOW) if it were counted; the real rows stay 0 + residual."""
+    n, h, w, cin, cout = 1, 9, 9, 64, 128                              # M = 81 < one row tile
+    numel = n * h * w * cout
+    x = torch.full((n * h * w * cin // (2 if a_bits == 4 else 1),), 0xFF if a_bits == 4 else -128,
+                   dtype=torch.uint8 if a_bits == 4 else torch.int8)
+    wt = torch.full((cout, 1, 1, cin), 127, dtype=torch.int8)
+    acc = cin * (15 if a_bits == 4 else -128) * 127
+    chan = ops.make_chan([-acc] * cout, [2 ** 31] * cout, [14] * cout)
+    d = ops.conv_desc(n, h, w, cin, cout, 1, 1, 1, 0, a_bits)
+    r = rng(a_bits)
+    res16 = torch.from_numpy(r.randint(0, 65536, size=numel).astype(np.uint16).view(np.int16))
+    res32 = rand_act(r, numel, 32)
+    for flags in (0, 1, 2):
+        for res, res_bits, y_bits, low_bits in [(res16, 16, 16, 8), (res32, 32, 32, 4)]:
+            ep = ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=0, res_bits=res_bits, res_me=RATIO_ONE, y_bits=y_bits, low_bits=low_bits,
+                              low_me=dyadic(0.003), low_clamp=(0, 15) if low_bits == 4 else (-128, 127), flags=flags)
+            cs, gs = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, res=res, out=out_buf(numel, y_bits),
+                                             out_low=out_buf(numel, low_bits)), ["out", "out_low"])
+            assert am.status["flags"] == 0
+            for a, b in zip(cs, gs):
+                assert torch.equal(a, b), (a_bits, flags, y_bits)
+        if flags:   # the resize-unit kernel: identity operand 0 on every row
+            x2 = torch.zeros_like(x)
+            w2 = torch.zeros((cout, 1, 1, cin), dtype=torch.int8)
+            chan2 = ops.make_chan([0] * cout, [2 ** 30] * cout, [31] * cout)
+            dd = ops.conv_desc(n, h, w, cin, cout, 1, 1, 1, 0, a_bits, 1)
+            ep = ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=1, res_bits=32, y_bits=16, low_bits=8, low_me=dyadic(0.003),
+                              low_clamp=(-128, 127), flags=flags)
+            args = dict(x=x, desc=dd, ep=ep, w=wt, chan=chan, desc2=dd, x2=x2, w2=w2, chan2=chan2, out=out_buf(numel, 16),
+                        out_low=out_buf(numel, 8))
+            cs, gs = run_both("conv2d_dual", args, ["out", "out_low"],
+                              gpu_overrides=dict(w=ops.upload_weights(wt, DEV), w2=ops.upload_weights(w2, DEV)))
+            assert am.status["flags"] == 0
+            for a, b in zip(cs, gs):
+                assert torch.equal(a, b), (a_bits, flags, "dual")
+
+
+@pytest.mark.parametrize("flags", [0, 1])
+def test_residual_stream_lands_on_65535_and_65536(flags):
+    """y = r + bias exactly (zero weights, both ratios exactly 1): 65535 fits the uint16 stream, 65536 raises
+    HAWQ_FLAG_RESIDUAL_OVERFLOW and is stored as 65535."""
+    n, h, w, cin, cout = 2, 9, 9, 64, 128                              # M = 162: one full and one ragged row tile
+    numel = n * h * w * cout
+    r = rng(65535 + flags)
+    x = rand_act(r, n * h * w * cin, 8)
+    wt = torch.zeros((cout, 1, 1, cin), dtype=torch.int8)
+    bias = r.randint(1, 30000, size=cout)
+    chan = ops.make_chan(bias, [2 ** 31] * cout, [31] * cout)
+    d = ops.conv_desc(n, h, w, cin, cout, 1, 1, 1, 0, 8)
+    for y, flag in [(65535, 0), (65536, 1)]:
+        res = torch.from_numpy(np.tile(y - bias, n * h * w).astype(np.uint16).view(np.int16))
+        ep = ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=0, res_bits=16, res_me=RATIO_ONE, y_bits=16, low_bits=8, low_me=dyadic(0.003),
+                          low_clamp=(-128, 127), flags=flags)
+        cs, gs = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, res=res, out=out_buf(numel, 16), out_low=out_buf(numel, 8)),
+                          ["out", "out_low"])
+        assert am.status["flags"] == flag
+        assert int((cs[0].to(torch.int32) & 0xFFFF).min()) == 65535
+        for a, b in zip(cs, gs):
+            assert torch.equal(a, b), (flags, y)
+
+
+@pytest.mark.parametrize("shape", [(130, 512, 999, 1024), (67, 192, 127, 128)])
+def test_linear_bias_edges(shape):
+    """DEQUANT_F32 tail at saturating biases and odd cout_store: the dp4a kernel (K % 128 == 0) and the convolution (other K)."""
+    nb, kk, co, cp = shape
+    r = rng(17 + nb + kk)
+    x = r.randint(-128, 128, size=(nb, kk))
+    x[0::3] = -128
+    x[1::3] = 127
+    wl = r.randint(-128, 128, size=(cp, kk))
+    for c in range(cp):
+        row = (-128, 127, -127, None)[(c // 8) % 4]
+        if row is not None:
+            wl[c] = row
+    wl[co:] = 0
+    edges = edge_biases(kk, 8)
+    chl = ops.make_chan([edges[c % 8] for c in range(cp)], [2 ** 30] * cp, [40] * cp)
+    fs = torch.from_numpy(r.uniform(1e-5, 1e-3, size=cp).astype(np.float32))
+    (c,), (g,) = run_both("linear", dict(x=torch.from_numpy(x.reshape(-1).astype(np.int8)), w=torch.from_numpy(wl.astype(np.int8)), chan=chl,
+                                         fscale=fs, out=torch.zeros((nb, co)), n=nb, k=kk, cout=co, cout_pad=cp), ["out"])
+    assert torch.equal(c, g), shape
+
+
+def test_requant_and_add_requant_stage1_bias_edges():
+    """requant / add_requant at ResNet-50 stage-1 size (batch 8, 56 x 56 x 256: the grid-stride loops run several times) with
+    int32-limit accumulators and biases."""
+    r = rng(56)
+    rows, ch = 8 * 56 * 56, 256
+    edges = [I32_MIN, I32_MIN + 1, I32_MAX, I32_MAX - 1, 2 ** 30, -2 ** 30, 0, 1]
+    me = [RATIO_ONE if c % 5 == 0 else dyadic([0.5, 0.25, 1.0, 3.0][c % 4] if c % 5 == 1 else float(np.exp(r.uniform(np.log(1e-9), 0.0))))
+          for c in range(ch)]
+    chan = ops.make_chan([edges[c % 8] if c % 2 else int(r.randint(-2 ** 20, 2 ** 20)) for c in range(ch)], [m for m, _ in me],
+                         [e for _, e in me])
+    acc = torch.from_numpy(r.randint(I32_MIN, I32_MAX, size=rows * ch, dtype=np.int64).astype(np.int32))
+    acc[:ch], acc[ch:2 * ch] = I32_MIN, I32_MAX
+    for x_bits, relu, out_bits in [(32, 1, 8), (32, 0, 16), (16, 1, 4), (32, 0, 8)]:
+        x = acc if x_bits == 32 else rand_act(r, rows * ch, 16)
+        clamp = {4: (0, 15), 8: (-128, 127), 16: (-32768, 32767)}[out_bits]
+        (a,), (b,) = run_both("requant", dict(x=x, rows=rows, c=ch, x_bits=x_bits, chan=chan, chan_stride=1, relu=relu, out_bits=out_bits,
+                                              clamp=clamp, out=out_buf(rows * ch, out_bits)), ["out"])
+        assert torch.equal(a, b), (x_bits, relu, out_bits)
+    res_chan = res_chan_with_ties(r, ch)
+    for res_kind, res_bits, y_bits, low_bits in [(0, 16, 16, 8), (1, 32, 32, 4), (0, 32, 16, 0), (1, 32, 16, 8)]:
+        if res_bits == 16:
+            res = torch.from_numpy(r.randint(0, 65536, size=rows * ch).astype(np.uint16).view(np.int16))
+        else:
+            res = torch.from_numpy(r.randint(I32_MIN, I32_MAX, size=rows * ch, dtype=np.int64).astype(np.int32))
+        ep = ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=res_kind, res_bits=res_bits, res_me=dyadic(0.6), y_bits=y_bits, low_bits=low_bits,
+                          low_me=dyadic(0.002), low_clamp=(0, 15) if low_bits == 4 else (-128, 127))
+        args = dict(acc=acc, rows=rows, c=ch, chan=chan, ep=ep, res=res, res_chan=res_chan if res_kind else None,
+                    y=out_buf(rows * ch, y_bits), out_low=out_buf(rows * ch, low_bits) if low_bits else None)
+        keys = [k for k in ("y", "out_low") if args[k] is not None]
+        cs, gs = run_both("add_requant", args, keys)
+        for a, b, k in zip(cs, gs, keys):
+            assert torch.equal(a, b), (res_kind, res_bits, y_bits, low_bits, k)
