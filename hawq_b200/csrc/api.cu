@@ -50,31 +50,40 @@ static int grid_for(long long work_items, int sm_count) {
   return (int)blocks;
 }
 
+// The maximum carveout lets the driver pick the 228 KB shared-memory configuration, the only one in which two CTAs of every
+// conv_igemm instantiation fit (ConvSmem's static_assert).
 template <int BN, bool A4, int EPI, bool DUAL>
 static int set_conv_attr1() {
   CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, EPI, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 ConvSmem<BN, A4, DUAL>::TOTAL));
+  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, EPI, DUAL>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                cudaSharedmemCarveoutMaxShared));
   return HAWQ_OK;
 }
 template <int BN, bool A4>
 static int set_conv_attr() {
   int rc;
   if ((rc = set_conv_attr1<BN, A4, EPI_GENERIC, false>()) || (rc = set_conv_attr1<BN, A4, EPI_FAST_LOW, false>()) ||
-      (rc = set_conv_attr1<BN, A4, EPI_FAST_RES, false>()) || (rc = set_conv_attr1<BN, A4, EPI_FAST_RES, true>()))
+      (rc = set_conv_attr1<BN, A4, EPI_FAST_RES, false>()))
     return rc;
   return HAWQ_OK;
 }
 
+// 1-D grid of (M / 128 row tiles) x (Cout / BN channel blocks), row tile major (conv_igemm_kernel derives m0, n0)
+static dim3 conv_grid(long long M, int Cout, int BN) { return dim3((unsigned)((M + CONV_BM - 1) / CONV_BM * (Cout / BN)), 1, 1); }
+
 template <int BN, bool A4>
-static void launch_conv(const ConvParams& p, dim3 grid, cudaStream_t s) {
+static void launch_conv(const ConvParams& p, cudaStream_t s) {
   const int smem = ConvSmem<BN, A4, false>::TOTAL;
+  const dim3 grid = conv_grid(p.M, p.Cout, BN);
   if (p.mode == HAWQ_EPI_REQUANT && p.out_bits <= 8) conv_igemm_kernel<BN, A4, EPI_FAST_LOW, false><<<grid, CONV_THREADS, smem, s>>>(p);
   else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, EPI_FAST_RES, false><<<grid, CONV_THREADS, smem, s>>>(p);
   else conv_igemm_kernel<BN, A4, EPI_GENERIC, false><<<grid, CONV_THREADS, smem, s>>>(p);
 }
-template <int BN, bool A4>
-static void launch_conv_dual(const ConvParams& p, dim3 grid, cudaStream_t s) {
-  conv_igemm_kernel<BN, A4, EPI_FAST_RES, true><<<grid, CONV_THREADS, ConvSmem<BN, A4, true>::TOTAL, s>>>(p);
+// resize units always run at BN = 64: the int32 identity tile of BN = 128 would leave room for one CTA per SM
+template <bool A4>
+static void launch_conv_dual(const ConvParams& p, cudaStream_t s) {
+  conv_igemm_kernel<64, A4, EPI_FAST_RES, true><<<conv_grid(p.M, p.Cout, 64), CONV_THREADS, ConvSmem<64, A4, true>::TOTAL, s>>>(p);
 }
 
 extern "C" {
@@ -98,7 +107,8 @@ int hawq_create(int device, hawq_handle** out) {
   int rc;
   CUDA_TRY(cudaFuncSetAttribute(linear_dp4a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, linear_smem_bytes(LIN_MAX_K)));
   if ((rc = set_conv_attr<128, false>()) || (rc = set_conv_attr<64, false>()) || (rc = set_conv_attr<128, true>()) ||
-      (rc = set_conv_attr<64, true>()))
+      (rc = set_conv_attr<64, true>()) || (rc = set_conv_attr1<64, false, EPI_FAST_RES, true>()) ||
+      (rc = set_conv_attr1<64, true, EPI_FAST_RES, true>()))
     return rc;
   *out = h;
   return HAWQ_OK;
@@ -220,16 +230,17 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
       return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: unknown epilogue mode %d", ep->mode);
   }
 
-  ++g_kernel_count[0];
   const bool bn128 = (d->Cout % 128 == 0);
-  const dim3 grid((unsigned)((M + CONV_BM - 1) / CONV_BM), (unsigned)(d->Cout / (bn128 ? 128 : 64)), 1);
+  if ((M + CONV_BM - 1) / CONV_BM * (d->Cout / (bn128 ? 128 : 64)) > 0x7fffffffll)
+    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: more than 2^31 - 1 output tiles");
+  ++g_kernel_count[0];
   cudaStream_t s = (cudaStream_t)stream;
   if (d->a_bits == 8) {
-    if (bn128) launch_conv<128, false>(p, grid, s);
-    else launch_conv<64, false>(p, grid, s);
+    if (bn128) launch_conv<128, false>(p, s);
+    else launch_conv<64, false>(p, s);
   } else {
-    if (bn128) launch_conv<128, true>(p, grid, s);
-    else launch_conv<64, true>(p, grid, s);
+    if (bn128) launch_conv<128, true>(p, s);
+    else launch_conv<64, true>(p, s);
   }
   return launch_check("conv_igemm");
 }
@@ -261,6 +272,8 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
   if (!ratios_one && !ratios_wide) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: needs a ratio-range promise (flags)");
   const long long M = (long long)d->N * d->H * d->W;
   if (M > 0x7fffff00ll || (long long)d2->N * d2->H * d2->W > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: too many pixels");
+  if ((M + CONV_BM - 1) / CONV_BM * (d->Cout / 64) > 0x7fffffffll)
+    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: more than 2^31 - 1 output tiles");
 
   ++g_kernel_count[4];
   ConvParams p;
@@ -275,16 +288,9 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
   p.x2 = (const uint8_t*)x2; p.w2 = w2; p.H2 = d2->H; p.W2 = d2->W; p.stride2 = d2->stride; p.cin_chunks2 = d2->Cin / 64;
   p.x2_pix_bytes = d2->Cin * d2->a_bits / 8;
 
-  const bool bn128 = (d->Cout % 128 == 0);
-  const dim3 grid((unsigned)((M + CONV_BM - 1) / CONV_BM), (unsigned)(d->Cout / (bn128 ? 128 : 64)), 1);
   cudaStream_t s = (cudaStream_t)stream;
-  if (d->a_bits == 8) {
-    if (bn128) launch_conv_dual<128, false>(p, grid, s);
-    else launch_conv_dual<64, false>(p, grid, s);
-  } else {
-    if (bn128) launch_conv_dual<128, true>(p, grid, s);
-    else launch_conv_dual<64, true>(p, grid, s);
-  }
+  if (d->a_bits == 8) launch_conv_dual<false>(p, s);
+  else launch_conv_dual<true>(p, s);
   return launch_check("conv_dual");
 }
 

@@ -58,6 +58,15 @@ constexpr int CONV_BM = 128;
 constexpr int CONV_STAGES = 4;
 constexpr int CONV_THREADS = 256;
 
+// Shared memory of one CTA.  The cp.async ring is free once the GEMM has drained, so the epilogue tiles reuse it:
+//   non-DUAL  [ ring | uint16 residual tile ] [ channel arrays ]
+//             The uint16 residual tile has its own region: it is prefetched while the ring is in use (see gemm()).
+//             After the GEMM the low-bit staging tile takes ring offset 0, and an int32 residual operand (loaded only after
+//             the GEMM) starts right behind it, across the rest of the ring and the uint16 region.
+//   DUAL      [ ring | int32 identity tile ] [ channel arrays ]
+//             The identity tile is written after the identity GEMM and read by the main convolution's epilogue.  After the
+//             main GEMM the low-bit tile (offset 0) and the uint16 stream tile (Y_OFF) are staged in the ring.
+// Two CTAs per SM (what __launch_bounds__(CONV_THREADS, 2) plans for) need 2 * (TOTAL + 1 KB reserved per CTA) <= 228 KB.
 template <int BN, bool A4, bool DUAL>
 struct ConvSmem {
   static constexpr int A_ROW = A4 ? 32 : 64;  // bytes of one A row per k-tile (64 channels)
@@ -65,18 +74,21 @@ struct ConvSmem {
   static constexpr int B_STAGE = BN * 64;
   static constexpr int PIPE = CONV_STAGES * (A_STAGE + B_STAGE);
   static constexpr int OUT_PITCH = BN + 16;
-  static constexpr int OUT_STAGE = CONV_BM * OUT_PITCH;
-  static constexpr int RES_TILE = CONV_BM * (BN * 4 + 32);                 // residual tile, worst case int32 + padding
-  // the residual / y tile reuses the pipeline ring, except in DUAL launches (filled before the main convolution's k loop)
-  static constexpr int RES_OFF = DUAL ? PIPE : 0;
-  static constexpr int MAIN = DUAL ? PIPE + RES_TILE : (PIPE > RES_TILE ? PIPE : RES_TILE);
-  static constexpr int OUT_OFF = MAIN;                                     // low-bit output staging tile
-  static constexpr int CHAN_OFF = OUT_OFF + OUT_STAGE;                     // hawq_chan[BN]
+  static constexpr int OUT_STAGE = CONV_BM * OUT_PITCH;                    // low-bit output staging tile, at offset 0
+  static constexpr int RES16 = CONV_BM * (BN * 2 + 16);                    // uint16 tile (residual operand or stream), padded pitch
+  static constexpr int RES32 = CONV_BM * (BN * 4 + 32);                    // int32 tile, padded pitch
+  static constexpr int RES16_OFF = PIPE;
+  static constexpr int RES32_OFF = DUAL ? PIPE : OUT_STAGE;
+  static constexpr int Y_OFF = OUT_STAGE;                                  // DUAL: staged uint16 stream tile
+  static constexpr int MAIN = DUAL ? PIPE + RES32 : (PIPE + RES16 > RES32_OFF + RES32 ? PIPE + RES16 : RES32_OFF + RES32);
+  static constexpr int CHAN_OFF = MAIN;                                    // hawq_chan[BN]
   static constexpr int M_OFF = CHAN_OFF + BN * (int)sizeof(hawq_chan);     // double[BN]: m * 2^-e of chan
   static constexpr int M1_OFF = M_OFF + BN * 8;                           // double[BN]: m * 2^-e of res_chan
   static constexpr int RC_OFF = M1_OFF + BN * 8;                          // hawq_chan[BN]: res_chan
   static constexpr int CB_OFF = RC_OFF + BN * (int)sizeof(hawq_chan);     // double[BN]: 2^52 + 2^31 - bias
   static constexpr int TOTAL = CB_OFF + BN * 8;
+  static_assert(OUT_STAGE <= PIPE && (!DUAL || Y_OFF + RES16 <= PIPE), "the epilogue staging tiles must fit in the freed ring");
+  static_assert(2 * (TOTAL + 1024) <= 228 * 1024, "two CTAs per SM must fit in shared memory");
 };
 
 // swizzled byte offset of 16-byte chunk `ch` of row `row` (rows of 64 B: 4 chunks; rows of 32 B: 2 chunks)
@@ -122,8 +134,11 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   const int lane = tid & 31, warp = tid >> 5;
   const int wg = warp >> 2;     // warpgroup: output rows 64 * wg ... 64 * wg + 63
   const int g = lane >> 2, t = lane & 3;
-  const int m0 = blockIdx.x * BM;
-  const int n0 = blockIdx.y * BN;
+  // 1-D grid, row tile major: the Cout / BN CTAs that read the same 128 activation rows are launched back to back, so all but
+  // the first find those rows in L2
+  const int nblk = p.Cout / BN;
+  const int m0 = (int)(blockIdx.x / nblk) * BM;
+  const int n0 = (int)(blockIdx.x % nblk) * BN;
 
   int slow = p.slow_scalar;
   int wide_bad = p.wide_scalar_bad;   // some ratio > 2^20: the FP64 FMA is no longer exact for every int32 operand
@@ -154,8 +169,27 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
 
   int32_t acc[NACC];
 
-  // acc = A(128 x K) * B(K x BN) of geometry gm for this CTA's tile
-  auto gemm = [&](const ConvGeom& gm) {
+  // RESIDUAL operand tile in shared memory; padded pitch keeps the fragment-pattern reads conflict-free
+  const int res_es = (p.mode == HAWQ_EPI_RESIDUAL) ? ((p.res_kind == 1 || p.res_bits == 32) ? 4 : 2) : 0;
+  const int res_pitch = BN * res_es + 8 * res_es;
+  uint8_t* sRes = smem + (res_es == 2 ? S::RES16_OFF : S::RES32_OFF);
+
+  // cp.async this CTA's tile of the residual operand into sRes (coalesced 16 B, zero-fill past M); no commit
+  auto load_res = [&]() {
+    const int cpr = BN * res_es / 16;   // 16-byte chunks per row
+    const uint8_t* gres = reinterpret_cast<const uint8_t*>(p.res);
+    for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
+      const int row = id / cpr, j = id - row * cpr;
+      const bool v = m0 + row < p.M;
+      const uint8_t* src = v ? gres + ((size_t)(m0 + row) * p.Cout + n0) * res_es + j * 16 : gres;
+      cp_async_16(smem_u32(sRes + row * res_pitch + j * 16), src, v ? 16 : 0);
+    }
+  };
+  // the uint16 residual operand has its own region: it is fetched while the GEMM runs (the int32 operand overlaps the ring)
+  const bool prefetch_res = !DUAL && res_es == 2;
+
+  // acc = A(128 x K) * B(K x BN) of geometry gm for this CTA's tile; with_res: the residual tile joins the prologue
+  auto gemm = [&](const ConvGeom& gm, bool with_res) {
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0;
     // per-thread gather coordinates for the A rows this thread copies
@@ -204,9 +238,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       }
     };
 
+    // cp.async groups retire in commit order.  The residual tile is issued right behind the prologue's k-tiles and
+    // committed in their last group (k-tile STAGES - 2), so it is in flight during the whole GEMM: the waits for k-tiles
+    // 0 ... STAGES - 3 never wait for it, and with KT < STAGES - 1 it is first waited for by the cp_async_wait<0> that
+    // ends the GEMM.  Committed as a group of its own it would add one group to every later wait (each k-tile waited
+    // for a stage early); committed first it would hold up k-tile 0.
 #pragma unroll
     for (int s = 0; s < STAGES - 1; ++s) {
       if (s < KT) load_tile(s);
+      if (s == STAGES - 2 && with_res) load_res();
       cp_async_commit();
     }
 
@@ -243,13 +283,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
     __syncthreads();   // pipeline buffers are free
   };
 
-  // RESIDUAL operand tile in shared memory; padded pitch keeps the fragment-pattern reads conflict-free
-  uint8_t* sRes = smem + S::RES_OFF;
-  const int res_es = (p.mode == HAWQ_EPI_RESIDUAL) ? ((p.res_kind == 1 || p.res_bits == 32) ? 4 : 2) : 0;
-  const int res_pitch = BN * res_es + 8 * res_es;
-
   if constexpr (DUAL) {   // identity convolution first: acc + bias2 (saturating) is the int32 res_kind 1 operand
-    gemm(ConvGeom{p.x2, p.w2, p.H2, p.W2, p.stride2, 0, 1, 1, p.cin_chunks2, p.x2_pix_bytes, p.cin_chunks2 * 64});
+    gemm(ConvGeom{p.x2, p.w2, p.H2, p.W2, p.stride2, 0, 1, 1, p.cin_chunks2, p.x2_pix_bytes, p.cin_chunks2 * 64}, false);
 #pragma unroll
     for (int ni = 0; ni < NT; ++ni) {
       const int col = ni * 8 + 2 * t;
@@ -262,27 +297,23 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       }
     }
   }
-  gemm(ConvGeom{p.x, p.w, p.H, p.W, p.stride, p.pad, p.KH, p.KW, p.cin_chunks, p.x_pix_bytes, p.K});
+  gemm(ConvGeom{p.x, p.w, p.H, p.W, p.stride, p.pad, p.KH, p.KW, p.cin_chunks, p.x_pix_bytes, p.K}, prefetch_res);
 
-  // RESIDUAL: bulk-load this tile of the residual operand (coalesced 16 B cp.async, zero-fill past M) instead of
-  // issuing dependent scalar loads inside the epilogue.
-  if (!DUAL && res_es) {
-    const int cpr = BN * res_es / 16;   // 16-byte chunks per row
-    const uint8_t* gres = reinterpret_cast<const uint8_t*>(p.res);
-    for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
-      const int row = id / cpr, j = id - row * cpr;
-      const bool v = m0 + row < p.M;
-      const uint8_t* src = v ? gres + ((size_t)(m0 + row) * p.Cout + n0) * res_es + j * 16 : gres;
-      cp_async_16(smem_u32(sRes + row * res_pitch + j * 16), src, v ? 16 : 0);
-    }
+  if (!DUAL && res_es == 4) {   // int32 residual operand: its tile overlaps the ring, so it is loaded now
+    load_res();
     cp_async_commit();
     cp_async_wait<0>();
     __syncthreads();
   }
-  const bool y_in_place = res_es != 0 && p.y_bits == res_es * 8;   // new residual stream overwrites the tile in smem
+  // the new residual stream is staged in shared memory and written with 16-byte stores: in place over the operand tile
+  // when both have the same width, in the freed ring in DUAL launches (uint16 stream over an int32 identity tile)
+  const bool y_staged = DUAL || (res_es != 0 && p.y_bits == res_es * 8);
+  const int y_es = p.y_bits / 8;
+  const int y_pitch = BN * y_es + 8 * y_es;
+  uint8_t* sY = DUAL ? smem + S::Y_OFF : sRes;
 
   // ------------------------------------------------------------------------------------------------ epilogue
-  uint8_t* sOut = smem + S::OUT_OFF;
+  uint8_t* sOut = smem;
   const bool stage_low = (p.mode == HAWQ_EPI_REQUANT && p.out_bits <= 8) || (p.mode == HAWQ_EPI_RESIDUAL && p.low_bits != 0);
   const int stage_bits = (p.mode == HAWQ_EPI_REQUANT) ? p.out_bits : p.low_bits;
 
@@ -362,14 +393,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
             }
             int y0 = max(sat_add(term(r0, M1.x, row_ok), v0), relu_floor);
             int y1 = max(sat_add(term(r1, M1.y, row_ok), v1), relu_floor);
+            uint8_t* yptr = sY + row * y_pitch + col * y_es;
             if (p.y_bits == 16) {
               if (row_ok) ymax = max(ymax, max(y0, y1));
               const uint32_t packed = (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
-              if (y_in_place) *reinterpret_cast<uint32_t*>(rptr) = packed;
+              if (y_staged) *reinterpret_cast<uint32_t*>(yptr) = packed;
               else if (m0 + row < p.M)
                 *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + (size_t)(m0 + row) * p.Cout + n0 + col) = packed;
             } else if (p.y_bits == 32) {
-              if (y_in_place) *reinterpret_cast<int2*>(rptr) = make_int2(y0, y1);
+              if (y_staged) *reinterpret_cast<int2*>(yptr) = make_int2(y0, y1);
               else if (m0 + row < p.M)
                 *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + (size_t)(m0 + row) * p.Cout + n0 + col) = make_int2(y0, y1);
             }
@@ -462,13 +494,14 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
             int32_t y0 = sat_add(rq_term(r0, rm0, re0, rM0, ok), rq_term(v0, (uint32_t)c0.y, c0.z, M01.x, ok));
             int32_t y1 = sat_add(rq_term(r1, rm1, re1, rM1, ok), rq_term(v1, (uint32_t)c1.y, c1.z, M01.y, ok));
             if (p.relu) { y0 = max(y0, 0); y1 = max(y1, 0); }
+            uint8_t* yptr = sY + row * y_pitch + col * y_es;
             if (p.y_bits == 32) {
-              if (y_in_place) *reinterpret_cast<int2*>(rptr) = make_int2(y0, y1);
+              if (y_staged) *reinterpret_cast<int2*>(yptr) = make_int2(y0, y1);
               else if (ok) *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + gidx) = make_int2(y0, y1);
             } else if (p.y_bits == 16) {
               if (ok && max(y0, y1) > 65535) atomicOr(p.status, HAWQ_FLAG_RESIDUAL_OVERFLOW);
               const uint32_t packed = (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
-              if (y_in_place) *reinterpret_cast<uint32_t*>(rptr) = packed;
+              if (y_staged) *reinterpret_cast<uint32_t*>(yptr) = packed;
               else if (ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + gidx) = packed;
             }
             if (p.low_bits != 0) {
@@ -496,15 +529,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
     else epilogue(std::true_type{});
   }
 
-  if (y_in_place || stage_low) __syncthreads();
-  if (y_in_place) {   // coalesced copy-out of the new residual stream tile
-    const int cpr = BN * res_es / 16;
+  if (y_staged || stage_low) __syncthreads();
+  if (y_staged) {   // coalesced copy-out of the new residual stream tile
+    const int cpr = BN * y_es / 16;
     uint8_t* gy = reinterpret_cast<uint8_t*>(p.out);
     for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
       const int row = id / cpr, j = id - row * cpr;
       if (m0 + row < p.M)
-        *reinterpret_cast<int4*>(gy + ((size_t)(m0 + row) * p.Cout + n0) * res_es + j * 16) =
-            *reinterpret_cast<const int4*>(sRes + row * res_pitch + j * 16);
+        *reinterpret_cast<int4*>(gy + ((size_t)(m0 + row) * p.Cout + n0) * y_es + j * 16) =
+            *reinterpret_cast<const int4*>(sY + row * y_pitch + j * 16);
     }
   }
   if (stage_low) {
