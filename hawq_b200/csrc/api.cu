@@ -52,19 +52,19 @@ static int grid_for(long long work_items, int sm_count) {
 
 // The maximum carveout lets the driver pick the 228 KB shared-memory configuration, the only one in which two CTAs of every
 // conv_igemm instantiation fit (ConvSmem's static_assert).
-template <int BN, bool A4, int EPI, bool DUAL>
+template <int BN, bool A4, int FAM, bool DUAL>
 static int set_conv_attr1() {
-  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, EPI, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, FAM, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 ConvSmem<BN, A4, DUAL>::TOTAL));
-  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, EPI, DUAL>, cudaFuncAttributePreferredSharedMemoryCarveout,
+  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, FAM, DUAL>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                 cudaSharedmemCarveoutMaxShared));
   return HAWQ_OK;
 }
 template <int BN, bool A4>
 static int set_conv_attr() {
   int rc;
-  if ((rc = set_conv_attr1<BN, A4, EPI_GENERIC, false>()) || (rc = set_conv_attr1<BN, A4, EPI_FAST_LOW, false>()) ||
-      (rc = set_conv_attr1<BN, A4, EPI_FAST_RES, false>()))
+  if ((rc = set_conv_attr1<BN, A4, FAM_REQUANT, false>()) || (rc = set_conv_attr1<BN, A4, FAM_RESIDUAL, false>()) ||
+      (rc = set_conv_attr1<BN, A4, FAM_STORE, false>()))
     return rc;
   return HAWQ_OK;
 }
@@ -76,14 +76,14 @@ template <int BN, bool A4>
 static void launch_conv(const ConvParams& p, cudaStream_t s) {
   const int smem = ConvSmem<BN, A4, false>::TOTAL;
   const dim3 grid = conv_grid(p.M, p.Cout, BN);
-  if (p.mode == HAWQ_EPI_REQUANT && p.out_bits <= 8) conv_igemm_kernel<BN, A4, EPI_FAST_LOW, false><<<grid, CONV_THREADS, smem, s>>>(p);
-  else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, EPI_FAST_RES, false><<<grid, CONV_THREADS, smem, s>>>(p);
-  else conv_igemm_kernel<BN, A4, EPI_GENERIC, false><<<grid, CONV_THREADS, smem, s>>>(p);
+  if (p.mode == HAWQ_EPI_REQUANT) conv_igemm_kernel<BN, A4, FAM_REQUANT, false><<<grid, CONV_THREADS, smem, s>>>(p);
+  else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, FAM_RESIDUAL, false><<<grid, CONV_THREADS, smem, s>>>(p);
+  else conv_igemm_kernel<BN, A4, FAM_STORE, false><<<grid, CONV_THREADS, smem, s>>>(p);
 }
 // resize units always run at BN = 64: the int32 identity tile of BN = 128 would leave room for one CTA per SM
 template <bool A4>
 static void launch_conv_dual(const ConvParams& p, cudaStream_t s) {
-  conv_igemm_kernel<64, A4, EPI_FAST_RES, true><<<conv_grid(p.M, p.Cout, 64), CONV_THREADS, ConvSmem<64, A4, true>::TOTAL, s>>>(p);
+  conv_igemm_kernel<64, A4, FAM_RESIDUAL, true><<<conv_grid(p.M, p.Cout, 64), CONV_THREADS, ConvSmem<64, A4, true>::TOTAL, s>>>(p);
 }
 
 extern "C" {
@@ -107,8 +107,8 @@ int hawq_create(int device, hawq_handle** out) {
   int rc;
   CUDA_TRY(cudaFuncSetAttribute(linear_dp4a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, linear_smem_bytes(LIN_MAX_K)));
   if ((rc = set_conv_attr<128, false>()) || (rc = set_conv_attr<64, false>()) || (rc = set_conv_attr<128, true>()) ||
-      (rc = set_conv_attr<64, true>()) || (rc = set_conv_attr1<64, false, EPI_FAST_RES, true>()) ||
-      (rc = set_conv_attr1<64, true, EPI_FAST_RES, true>()))
+      (rc = set_conv_attr<64, true>()) || (rc = set_conv_attr1<64, false, FAM_RESIDUAL, true>()) ||
+      (rc = set_conv_attr1<64, true, FAM_RESIDUAL, true>()))
     return rc;
   *out = h;
   return HAWQ_OK;
@@ -143,10 +143,10 @@ int hawq_copy_status(hawq_handle* h, int32_t* dst, void* stream) {
 }
 
 // |acc| <= K * 128 * 128 (int8 activations) or K * 15 * 128 (unsigned 4-bit activations), int8 weights: a bias in
-// [bias_lo, bias_hi] keeps acc + bias inside int32, so the fast epilogues may add it without saturating
+// [bias_lo, bias_hi] keeps acc + bias inside int32, so the FP64 epilogue needs no clamp
 static void set_bias_window(ConvParams& p, int a_bits) {
   long long bound = (long long)p.K * (a_bits == 4 ? 15 * 128 : 128 * 128);
-  if (bound > 2147483648ll) bound = 2147483648ll;   // empty window: every bias takes the saturating epilogue
+  if (bound > 2147483648ll) bound = 2147483648ll;   // empty window: every FP64 CTA clamps acc + bias
   p.bias_lo = (int)(bound - 2147483648ll);
   p.bias_hi = (int)(2147483647ll - bound);
 }
@@ -184,12 +184,11 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
   p.y_bits = ep->y_bits; p.low_bits = ep->low_bits; p.low_m = ep->low_m; p.low_e = ep->low_e;
   p.low_lo = ep->low_lo; p.low_hi = ep->low_hi; p.cout_store = ep->cout_store;
   set_bias_window(p, d->a_bits);
-  p.slow_scalar = 0;
   p.check_ovf = ep->mode == HAWQ_EPI_RESIDUAL && (ep->flags & (HAWQ_EP_RATIOS_LE_ONE | HAWQ_EP_RATIOS_LE_2P20)) != 0;
-  if (ep->mode == HAWQ_EPI_RESIDUAL) {
-    if (ep->res_kind == 0 && !dyadic_is_fast(ep->res_m, ep->res_e)) p.slow_scalar = 1;
-    if (ep->low_bits != 0 && !dyadic_is_fast(ep->low_m, ep->low_e)) p.slow_scalar = 1;
-    p.wide_scalar_bad = (ep->res_kind == 0 && !dyadic_is_wide(ep->res_m, ep->res_e)) || (ep->low_bits != 0 && !dyadic_is_fast(ep->low_m, ep->low_e));
+  if (ep->mode == HAWQ_EPI_RESIDUAL) {   // the scalar ratios' part of the kernel's per-CTA requantisation policy
+    const bool low_over_one = ep->low_bits != 0 && !dyadic_is_fast(ep->low_m, ep->low_e);
+    p.scalar_over_one = (ep->res_kind == 0 && !dyadic_is_fast(ep->res_m, ep->res_e)) || low_over_one;
+    p.scalar_unchecked = (ep->res_kind == 0 && !dyadic_is_wide(ep->res_m, ep->res_e)) || low_over_one;
   }
 
   switch (ep->mode) {

@@ -13,8 +13,10 @@
 //   DUAL = true (resize units): the identity-branch 1x1 convolution (x2, w2) runs first in the same CTA; its int32 result
 //   (acc + bias2) stays in shared memory as the res_kind 1 operand of the RESIDUAL epilogue of the main convolution.
 //
-//   Epilogues (hawq_epilogue_mode): REQUANT (case 0 of fixedpoint_fn), RESIDUAL (case 1: dual dyadic requant + add,
-//   optional ReLU, writes the new residual stream and/or the next unit's low-bit activation), RAW_I32, DEQUANT_F32.
+//   Epilogues (hawq_epilogue_mode), one instantiation per family: REQUANT (case 0 of fixedpoint_fn), RESIDUAL (case 1: dual
+//   dyadic requant + add, optional ReLU, writes the new residual stream and/or the next unit's low-bit activation), and STORE
+//   (RAW_I32, DEQUANT_F32).  The REQUANT and RESIDUAL bodies are written once, over a requantisation implementation that each
+//   CTA picks from its channels' ratios and biases (RqFp64: one FP64 FMA per term; RqExact: 64-bit integer arithmetic).
 #pragma once
 #include <type_traits>
 
@@ -44,8 +46,8 @@ struct ConvParams {
   uint32_t low_m;
   int low_e, low_lo, low_hi;
   int cout_store;
-  int slow_scalar;   // host-checked: a scalar dyadic pair (res / low) has ratio > 1 -> generic 64-bit requant
-  int wide_scalar_bad;   // host-checked: the scalar residual ratio exceeds 2^20 or the low-bit ratio exceeds 1 (no WIDE epilogue)
+  int scalar_over_one;   // host-checked: a scalar dyadic pair (res / low) has ratio > 1
+  int scalar_unchecked;  // host-checked: the scalar residual ratio exceeds 2^20 or the low-bit ratio exceeds 1 (no checked FP64 form)
   int check_ovf;     // RESIDUAL under a HAWQ_EP_RATIOS_* promise: a requantised term leaving int32 raises HAWQ_FLAG_REQUANT_OVERFLOW
   int bias_lo, bias_hi;   // host-computed from K and a_bits: a bias in [bias_lo, bias_hi] keeps acc + bias inside int32 (empty when bias_lo > bias_hi)
   // DUAL launches: the identity 1x1 convolution (res_chan holds its bias and per-channel identity ratio)
@@ -98,9 +100,55 @@ __device__ __forceinline__ int swz(int row, int ch) {
   else return row * 32 + ((ch ^ ((row >> 2) & 1)) << 4);
 }
 
-// EPI selects the compile-time specialised fast epilogue (used when every dyadic ratio of the CTA is <= 1 and every bias keeps
-// acc + bias inside int32, which the kernel verifies): 0 = none (generic run-time epilogue only), 1 = REQUANT to 4/8 bits, 2 = RESIDUAL.
-constexpr int EPI_GENERIC = 0, EPI_FAST_LOW = 1, EPI_FAST_RES = 2;
+// Epilogue family of an instantiation (FAM): REQUANT to 4/8/16/32 bits, RESIDUAL (DUAL launches included), STORE (RAW_I32 and
+// DEQUANT_F32, no requantisation).  A kernel carries its own family's body only.
+constexpr int FAM_REQUANT = 0, FAM_RESIDUAL = 1, FAM_STORE = 2;
+
+// One requantised term q = RHE(value * m / 2^e) of an epilogue, in one of two implementations; the kernel picks one per CTA.
+// Operands are built by acc_bias (acc + bias of a channel), of_i32 and of_u16; term() takes the ratio both as M = m * 2^-e and as
+// (m, e), and with `count` set a result outside int32 raises HAWQ_FLAG_REQUANT_OVERFLOW when the CTA is `checked`.
+//
+// FP64: an operand is its value as an exact double, built from bits without a conversion instruction ({0x43300000, v ^ 0x80000000}
+// is 2^52 + 2^31 + v; the channel's sCb = 2^52 + 2^31 - bias folds the bias add into it).  t = fma(d, M, 1.5 * 2^52) rounds the
+// exact product once, ties to even, and its low word is q whenever |d * M| < 2^51: always for ratios <= 1 (|q| <= |d| <= 2^31).
+// For ratios up to 2^20 (checked) d * M is still exact inside the FMA and t - 1.5 * 2^52 is exact while q fits int32 and far outside
+// int32 otherwise, so one compare pair detects every overflow.  CLAMPED: some bias of the CTA can take acc + bias out of int32, so
+// that sum is clamped to int32 (d is exact, so the clamp equals sat_add); a compile-time flag keeps the clamp off the common path.
+template <bool CLAMPED>
+struct RqFp64 {
+  bool checked;
+  bool ovf = false;
+  static constexpr double kMagic = 6755399441055744.0;   // 1.5 * 2^52
+  __device__ static double acc_bias(int32_t acc, double cb, int32_t) {
+    const double d = __hiloint2double(0x43300000, acc ^ 0x80000000) - cb;
+    return CLAMPED ? fmin(fmax(d, -2147483648.0), 2147483647.0) : d;
+  }
+  __device__ static double of_i32(int32_t v) {
+    return __hiloint2double(0x43300000, v ^ 0x80000000) - 4503601774854144.0;   // - (2^52 + 2^31)
+  }
+  __device__ static double of_u16(uint32_t u) { return __hiloint2double(0x43300000, (int)u) - 4503599627370496.0; }   // - 2^52
+  __device__ int32_t term(double d, double M, uint32_t, int32_t, bool count) {
+    const double t = __fma_rn(d, M, kMagic);
+    if (checked && count) {
+      const double q = t - kMagic;
+      ovf |= q > 2147483647.0 || q < -2147483648.0;
+    }
+    return __double2loint(t);
+  }
+};
+// Exact: rhe_requant64 of the saturated int32 value, for any ratio, saturated to int32.
+struct RqExact {
+  bool checked;
+  bool ovf = false;
+  __device__ static int32_t acc_bias(int32_t acc, double, int32_t bias) { return sat_add(acc, bias); }
+  __device__ static int32_t of_i32(int32_t v) { return v; }
+  __device__ static int32_t of_u16(uint32_t u) { return (int32_t)u; }
+  __device__ int32_t term(int32_t v, double, uint32_t m, int32_t e, bool count) {
+    const long long q = rhe_requant64(v, m, e);
+    if (checked && count) ovf |= q > 2147483647ll || q < -2147483648ll;
+    return sat_i32(q);
+  }
+};
 
 // geometry of one implicit GEMM of a launch (the main convolution, or the identity convolution of a DUAL launch)
 struct ConvGeom {
@@ -109,7 +157,7 @@ struct ConvGeom {
   int H, W, stride, pad, KH, KW, cin_chunks, x_pix_bytes, K;
 };
 
-template <int BN, bool A4, int EPI, bool DUAL>
+template <int BN, bool A4, int FAM, bool DUAL>
 __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvParams p) {
   using S = ConvSmem<BN, A4, DUAL>;
   constexpr int BM = CONV_BM, STAGES = CONV_STAGES;
@@ -140,49 +188,50 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   const int m0 = (int)(blockIdx.x / nblk) * BM;
   const int n0 = (int)(blockIdx.x % nblk) * BN;
 
-  int slow = p.slow_scalar;
-  int wide_bad = p.wide_scalar_bad;   // some ratio > 2^20: the FP64 FMA is no longer exact for every int32 operand
-  int bias_wide = 0;                  // some acc + bias may leave int32: the folded (unsaturated) bias add would differ from sat_add
+  int over_one = p.scalar_over_one;     // some ratio > 1
+  int unchecked = p.scalar_unchecked;   // some ratio > 2^20 (or a low-bit ratio > 1): beyond the checked FP64 form
+  int bias_out = 0;                     // some bias outside [bias_lo, bias_hi]: acc + bias may leave int32
   if (tid < BN) {
     const hawq_chan c = p.chan[n0 + tid];
     sChan[tid] = c;
     sM[tid] = dyadic_to_double(c.m, c.e);
     sCb[tid] = 4503601774854144.0 - (double)c.bias;   // exact: folds the bias add into the int -> double conversion
-    bias_wide = c.bias < p.bias_lo || c.bias > p.bias_hi;
-    slow |= !dyadic_is_fast(c.m, c.e);
-    wide_bad |= !dyadic_is_wide(c.m, c.e);
-    if (p.mode == HAWQ_EPI_RESIDUAL && p.res_kind == 1) {
+    bias_out = c.bias < p.bias_lo || c.bias > p.bias_hi;
+    over_one |= !dyadic_is_fast(c.m, c.e);
+    unchecked |= !dyadic_is_wide(c.m, c.e);
+    if (FAM == FAM_RESIDUAL && p.res_kind == 1) {
       const hawq_chan rc = p.res_chan[n0 + tid];
       sResChan[tid] = rc;
       sM1[tid] = dyadic_to_double(rc.m, rc.e);
-      slow |= !dyadic_is_fast(rc.m, rc.e);
-      wide_bad |= !dyadic_is_wide(rc.m, rc.e);
+      over_one |= !dyadic_is_fast(rc.m, rc.e);
+      unchecked |= !dyadic_is_wide(rc.m, rc.e);
     }
   }
-  const bool use_slow = __syncthreads_or(slow) != 0;   // CTA-uniform: any ratio > 1 -> generic exact integer requant
-  // RESIDUAL under a ratio promise with every ratio <= 2^20: the FP64 epilogue stays exact whenever a term fits int32, and every term
-  // is range-checked (HAWQ_FLAG_REQUANT_OVERFLOW), so it replaces the generic epilogue (CTA-uniform)
-  const bool use_wide = (__syncthreads_or(wide_bad) == 0) && use_slow && p.check_ovf && p.mode == HAWQ_EPI_RESIDUAL;
-  // the specialised epilogues add the bias without saturating (sCb); a CTA with a bias near the int32 limits takes the
-  // sat_add epilogue instead (CTA-uniform)
-  const bool bias_fold = __syncthreads_or(bias_wide) == 0;
+  // Requantisation policy, CTA-uniform: FP64 when every ratio is <= 1, and for RESIDUAL under a ratio promise when every ratio is
+  // <= 2^20 (the low-bit ratio <= 1), each term then checked; Exact otherwise.  An FP64 CTA with a bias outside the window clamps.
+  const bool ratio_over_one = __syncthreads_or(over_one) != 0;
+  const bool ratio_unchecked = __syncthreads_or(unchecked) != 0;
+  const bool clamped = __syncthreads_or(bias_out) != 0;
+  const bool fp64 = !ratio_over_one || (FAM == FAM_RESIDUAL && p.check_ovf && !ratio_unchecked);
 
   int32_t acc[NACC];
 
   // RESIDUAL operand tile in shared memory; padded pitch keeps the fragment-pattern reads conflict-free
-  const int res_es = (p.mode == HAWQ_EPI_RESIDUAL) ? ((p.res_kind == 1 || p.res_bits == 32) ? 4 : 2) : 0;
+  const int res_es = (FAM == FAM_RESIDUAL) ? ((p.res_kind == 1 || p.res_bits == 32) ? 4 : 2) : 0;
   const int res_pitch = BN * res_es + 8 * res_es;
   uint8_t* sRes = smem + (res_es == 2 ? S::RES16_OFF : S::RES32_OFF);
 
   // cp.async this CTA's tile of the residual operand into sRes (coalesced 16 B, zero-fill past M); no commit
   auto load_res = [&]() {
-    const int cpr = BN * res_es / 16;   // 16-byte chunks per row
-    const uint8_t* gres = reinterpret_cast<const uint8_t*>(p.res);
-    for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
-      const int row = id / cpr, j = id - row * cpr;
-      const bool v = m0 + row < p.M;
-      const uint8_t* src = v ? gres + ((size_t)(m0 + row) * p.Cout + n0) * res_es + j * 16 : gres;
-      cp_async_16(smem_u32(sRes + row * res_pitch + j * 16), src, v ? 16 : 0);
+    if constexpr (FAM == FAM_RESIDUAL) {
+      const int cpr = BN * res_es / 16;   // 16-byte chunks per row
+      const uint8_t* gres = reinterpret_cast<const uint8_t*>(p.res);
+      for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
+        const int row = id / cpr, j = id - row * cpr;
+        const bool v = m0 + row < p.M;
+        const uint8_t* src = v ? gres + ((size_t)(m0 + row) * p.Cout + n0) * res_es + j * 16 : gres;
+        cp_async_16(smem_u32(sRes + row * res_pitch + j * 16), src, v ? 16 : 0);
+      }
     }
   };
   // the uint16 residual operand has its own region: it is fetched while the GEMM runs (the int32 operand overlaps the ring)
@@ -314,219 +363,130 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
 
   // ------------------------------------------------------------------------------------------------ epilogue
   uint8_t* sOut = smem;
-  const bool stage_low = (p.mode == HAWQ_EPI_REQUANT && p.out_bits <= 8) || (p.mode == HAWQ_EPI_RESIDUAL && p.low_bits != 0);
-  const int stage_bits = (p.mode == HAWQ_EPI_REQUANT) ? p.out_bits : p.low_bits;
+  const bool stage_low = (FAM == FAM_REQUANT && p.out_bits <= 8) || (FAM == FAM_RESIDUAL && p.low_bits != 0);
+  const int stage_bits = (FAM == FAM_REQUANT) ? p.out_bits : p.low_bits;
 
-  constexpr double kMagic = 6755399441055744.0;      // 1.5 * 2^52
-  constexpr double kOffS = 4503601774854144.0;       // 2^52 + 2^31 (signed int -> double)
-  constexpr double kOffU = 4503599627370496.0;       // 2^52        (non-negative int -> double)
-  bool fast_done = false;
+  // a pair of low-bit outputs (columns col, col + 1) into the staging tile
+  auto put_low = [&](int row, int col, int q0, int q1) {
+    *reinterpret_cast<uint16_t*>(sOut + row * S::OUT_PITCH + col) = (uint16_t)__byte_perm(q0, q1, 0x0040);
+  };
+  // a pair of the new residual stream, staged or stored directly; a uint16 stream saturates at 65535, and ymax keeps the largest
+  // value of the thread's real rows for HAWQ_FLAG_RESIDUAL_OVERFLOW
+  auto put_y = [&](int row, int col, bool ok, int y0, int y1, int& ymax) {
+    if (p.y_bits == 16 && ok) ymax = max(ymax, max(y0, y1));
+    if (!y_staged && !ok) return;
+    uint8_t* dst = y_staged ? sY + row * y_pitch + col * y_es
+                            : reinterpret_cast<uint8_t*>(p.out) + ((size_t)(m0 + row) * p.Cout + n0 + col) * y_es;
+    if (p.y_bits == 16) *reinterpret_cast<uint32_t*>(dst) = (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
+    else if (p.y_bits == 32) *reinterpret_cast<int2*>(dst) = make_int2(y0, y1);
+  };
 
-  if constexpr (EPI == EPI_FAST_LOW) {
-    if (!use_slow && bias_fold) {
-      fast_done = true;
-      // clamp(RHE((acc + bias) * M)), ReLU folded into the lower clamp bound (RHE is monotone, RHE(0) = 0)
-      const int lo = p.relu ? max(p.lo, 0) : p.lo, hi = p.hi;
+  // the REQUANT or RESIDUAL body over one requantisation implementation (RqFp64 or RqExact); REQUANT is compiled separately for
+  // 4/8-bit outputs (staged) and 16/32-bit outputs (stored directly), so that no store branch splits the unrolled loop and the
+  // terms' FP64 latencies overlap
+  auto epilogue = [&](auto rq, auto low_out) {
+    if constexpr (FAM == FAM_REQUANT) {
+      // clamp(RHE((acc + bias) * ratio)), ReLU folded into the lower clamp bound (both implementations are monotone with RHE(0) = 0)
+      const int lo = p.relu ? min(max(p.lo, 0), p.hi) : p.lo;
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
         const int col = ni * 8 + 2 * t;
-        const double2 Cb = *reinterpret_cast<const double2*>(&sCb[col]);
+        const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);   // bias, m, e
+        const int4 c1 = *reinterpret_cast<const int4*>(&sChan[col + 1]);
         const double2 M = *reinterpret_cast<const double2*>(&sM[col]);
-        {
+        const double2 Cb = *reinterpret_cast<const double2*>(&sCb[col]);
 #pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            const int row = warp * 16 + hf * 8 + g;
-            const double d0 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 0] ^ 0x80000000) - Cb.x;
-            const double d1 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 1] ^ 0x80000000) - Cb.y;
-            const int q0 = clampi(__double2loint(__fma_rn(d0, M.x, kMagic)), lo, hi);
-            const int q1 = clampi(__double2loint(__fma_rn(d1, M.y, kMagic)), lo, hi);
-            *reinterpret_cast<uint16_t*>(sOut + row * S::OUT_PITCH + col) = (uint16_t)__byte_perm(q0, q1, 0x0040);
+        for (int hf = 0; hf < 2; ++hf) {
+          const int row = warp * 16 + hf * 8 + g;
+          const int q0 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2], Cb.x, c0.x), M.x, c0.y, c0.z, false), lo, p.hi);
+          const int q1 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2 + 1], Cb.y, c1.x), M.y, c1.y, c1.z, false), lo, p.hi);
+          if constexpr (decltype(low_out)::value) {
+            put_low(row, col, q0, q1);
+          } else if (m0 + row < p.M) {
+            uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)(m0 + row) * p.Cout + n0 + col) * (p.out_bits / 8);
+            if (p.out_bits == 16) *reinterpret_cast<uint32_t*>(dst) = (uint32_t)(q0 & 0xFFFF) | ((uint32_t)q1 << 16);
+            else *reinterpret_cast<int2*>(dst) = make_int2(q0, q1);
           }
         }
       }
-    }
-  }
-
-  if constexpr (EPI == EPI_FAST_RES) {
-    if (bias_fold && (!use_slow || use_wide)) {
-      fast_done = true;
-      // t = fma(d, M, 1.5 * 2^52) with d * M exact inside the FMA: for |d * M| < 2^51 the low word of t is RHE(d * M); a term outside
-      // int32 (which includes every |d * M| >= 2^51) is detected on t - 1.5 * 2^52 (exact in range, far out of range otherwise)
-      bool ovf = false;
-      auto term = [&](double d, double Mx, bool row_ok) -> int {
-        const double tt = __fma_rn(d, Mx, kMagic);
-        if (use_wide) {
-          const double q = tt - kMagic;
-          ovf |= row_ok && (q > 2147483647.0 || q < -2147483648.0);
-        }
-        return __double2loint(tt);
-      };
+    } else {
+      // y = [ReLU](sat_add(RHE(r * ratio1), RHE((acc + bias) * ratio))), the new stream and/or the low-bit copy clamp(RHE(y * low ratio))
       const double res_M = dyadic_to_double(p.res_m, p.res_e), low_M = dyadic_to_double(p.low_m, p.low_e);
       const int relu_floor = p.relu ? 0 : (int)0x80000000;
       int ymax = 0;
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
         const int col = ni * 8 + 2 * t;
-        const double2 Cb = *reinterpret_cast<const double2*>(&sCb[col]);
+        const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);   // bias, m, e
+        const int4 c1 = *reinterpret_cast<const int4*>(&sChan[col + 1]);
         const double2 M = *reinterpret_cast<const double2*>(&sM[col]);
-        double2 M1 = make_double2(res_M, res_M);
-        if (p.res_kind == 1) M1 = *reinterpret_cast<const double2*>(&sM1[col]);
-        {
+        const double2 Cb = *reinterpret_cast<const double2*>(&sCb[col]);
+        double2 M1 = make_double2(res_M, res_M);   // the residual operand's ratio: scalar or per channel
+        uint2 m1 = make_uint2(p.res_m, p.res_m);
+        int2 e1 = make_int2(p.res_e, p.res_e);
+        if (p.res_kind == 1) {
+          M1 = *reinterpret_cast<const double2*>(&sM1[col]);
+          m1 = make_uint2(sResChan[col].m, sResChan[col + 1].m);
+          e1 = make_int2(sResChan[col].e, sResChan[col + 1].e);
+        }
 #pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            const int row = warp * 16 + hf * 8 + g;
-            const bool row_ok = m0 + row < p.M;
-            const double d0 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 0] ^ 0x80000000) - Cb.x;
-            const double d1 = __hiloint2double(0x43300000, acc[ni * 4 + hf * 2 + 1] ^ 0x80000000) - Cb.y;
-            const int v0 = term(d0, M.x, row_ok);
-            const int v1 = term(d1, M.y, row_ok);
-            uint8_t* rptr = sRes + row * res_pitch + col * res_es;
-            double r0, r1;
-            if (res_es == 2) {   // uint16 residual stream: non-negative, no sign fix-up
-              const uint32_t pr = *reinterpret_cast<const uint32_t*>(rptr);
-              r0 = __hiloint2double(0x43300000, (int)(pr & 0xFFFFu)) - kOffU;
-              r1 = __hiloint2double(0x43300000, (int)(pr >> 16)) - kOffU;
-            } else {
-              const int2 pr = *reinterpret_cast<const int2*>(rptr);
-              r0 = __hiloint2double(0x43300000, pr.x ^ 0x80000000) - kOffS;
-              r1 = __hiloint2double(0x43300000, pr.y ^ 0x80000000) - kOffS;
-            }
-            int y0 = max(sat_add(term(r0, M1.x, row_ok), v0), relu_floor);
-            int y1 = max(sat_add(term(r1, M1.y, row_ok), v1), relu_floor);
-            uint8_t* yptr = sY + row * y_pitch + col * y_es;
-            if (p.y_bits == 16) {
-              if (row_ok) ymax = max(ymax, max(y0, y1));
-              const uint32_t packed = (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
-              if (y_staged) *reinterpret_cast<uint32_t*>(yptr) = packed;
-              else if (m0 + row < p.M)
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + (size_t)(m0 + row) * p.Cout + n0 + col) = packed;
-            } else if (p.y_bits == 32) {
-              if (y_staged) *reinterpret_cast<int2*>(yptr) = make_int2(y0, y1);
-              else if (m0 + row < p.M)
-                *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + (size_t)(m0 + row) * p.Cout + n0 + col) = make_int2(y0, y1);
-            }
-            if (p.low_bits != 0) {
-              const double l0 = __hiloint2double(0x43300000, y0 ^ 0x80000000) - kOffS;
-              const double l1 = __hiloint2double(0x43300000, y1 ^ 0x80000000) - kOffS;
-              const int q0 = clampi(__double2loint(__fma_rn(l0, low_M, kMagic)), p.low_lo, p.low_hi);
-              const int q1 = clampi(__double2loint(__fma_rn(l1, low_M, kMagic)), p.low_lo, p.low_hi);
-              *reinterpret_cast<uint16_t*>(sOut + row * S::OUT_PITCH + col) = (uint16_t)__byte_perm(q0, q1, 0x0040);
-            }
+        for (int hf = 0; hf < 2; ++hf) {
+          const int row = warp * 16 + hf * 8 + g;
+          const bool ok = m0 + row < p.M;
+          const uint8_t* rptr = sRes + row * res_pitch + col * res_es;
+          decltype(rq.of_i32(0)) r0, r1;
+          if (res_es == 2) {   // uint16 residual stream
+            const uint32_t pr = *reinterpret_cast<const uint32_t*>(rptr);
+            r0 = rq.of_u16(pr & 0xFFFFu);
+            r1 = rq.of_u16(pr >> 16);
+          } else {
+            const int2 pr = *reinterpret_cast<const int2*>(rptr);
+            r0 = rq.of_i32(pr.x);
+            r1 = rq.of_i32(pr.y);
           }
+          const auto v0 = rq.acc_bias(acc[ni * 4 + hf * 2 + 0], Cb.x, c0.x);
+          const auto v1 = rq.acc_bias(acc[ni * 4 + hf * 2 + 1], Cb.y, c1.x);
+          const int y0 = max(sat_add(rq.term(r0, M1.x, m1.x, e1.x, ok), rq.term(v0, M.x, c0.y, c0.z, ok)), relu_floor);
+          const int y1 = max(sat_add(rq.term(r1, M1.y, m1.y, e1.y, ok), rq.term(v1, M.y, c1.y, c1.z, ok)), relu_floor);
+          put_y(row, col, ok, y0, y1, ymax);
+          if (p.low_bits != 0)
+            put_low(row, col, clampi(rq.term(rq.of_i32(y0), low_M, p.low_m, p.low_e, false), p.low_lo, p.low_hi),
+                    clampi(rq.term(rq.of_i32(y1), low_M, p.low_m, p.low_e, false), p.low_lo, p.low_hi));
         }
       }
-      if (p.y_bits == 16 && ymax > 65535) atomicOr(p.status, HAWQ_FLAG_RESIDUAL_OVERFLOW);
-      if (ovf) atomicOr(p.status, HAWQ_FLAG_REQUANT_OVERFLOW);
+      if (ymax > 65535) atomicOr(p.status, HAWQ_FLAG_RESIDUAL_OVERFLOW);
+      if (rq.ovf) atomicOr(p.status, HAWQ_FLAG_REQUANT_OVERFLOW);
     }
-  }
+  };
 
-  auto epilogue = [&](auto fast_tag) {
-    constexpr bool FAST = decltype(fast_tag)::value;
-    const double res_M = dyadic_to_double(p.res_m, p.res_e), low_M = dyadic_to_double(p.low_m, p.low_e);
-    auto rq = [&](int32_t v, uint32_t m, int e, double M) -> int32_t {
-      if constexpr (FAST) return rhe_requant_fast(v, M);
-      else return rhe_requant(v, m, e);
-    };
-    // the two terms of a RESIDUAL sum: under a ratio promise (check_ovf) a term outside int32 raises HAWQ_FLAG_REQUANT_OVERFLOW
-    // (ratios <= 1, the FAST case, cannot leave int32)
-    bool ovf = false;
-    auto rq_term = [&](int32_t v, uint32_t m, int e, double M, bool row_ok) -> int32_t {
-      if constexpr (FAST) {
-        return rhe_requant_fast(v, M);
-      } else {
-        const long long q = rhe_requant64(v, m, e);
-        ovf |= row_ok && (q > 2147483647ll || q < -2147483648ll);
-        return sat_i32(q);
-      }
-    };
-    {
+  if constexpr (FAM == FAM_STORE) {   // RAW_I32: sat_add(acc, bias); DEQUANT_F32: float(acc + bias) * fscale, first cout_store columns
+#pragma unroll
+    for (int ni = 0; ni < NT; ++ni) {
+      const int col = ni * 8 + 2 * t;
+      const int b0 = sChan[col].bias, b1 = sChan[col + 1].bias;
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
-        const int row = warp * 16 + hf * 8 + g;
-        const int m = m0 + row;
-        const bool ok = m < p.M;
-#pragma unroll
-        for (int ni = 0; ni < NT; ++ni) {
-          const int col = ni * 8 + 2 * t;
-          const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);
-          const int4 c1 = *reinterpret_cast<const int4*>(&sChan[col + 1]);
-          const double2 M01 = *reinterpret_cast<const double2*>(&sM[col]);
-          int32_t v0 = sat_add(acc[ni * 4 + hf * 2 + 0], c0.x);
-          int32_t v1 = sat_add(acc[ni * 4 + hf * 2 + 1], c1.x);
-          const size_t gidx = (size_t)m * p.Cout + n0 + col;
-          if (p.mode == HAWQ_EPI_REQUANT) {
-            if (p.relu) { v0 = max(v0, 0); v1 = max(v1, 0); }
-            const int32_t q0 = clampi(rq(v0, (uint32_t)c0.y, c0.z, M01.x), p.lo, p.hi);
-            const int32_t q1 = clampi(rq(v1, (uint32_t)c1.y, c1.z, M01.y), p.lo, p.hi);
-            if (p.out_bits <= 8) {
-              *reinterpret_cast<uint16_t*>(sOut + row * S::OUT_PITCH + col) = (uint16_t)((q0 & 0xFF) | ((q1 & 0xFF) << 8));
-            } else if (ok) {
-              if (p.out_bits == 16) {
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<int16_t*>(p.out) + gidx) =
-                    (uint32_t)(q0 & 0xFFFF) | ((uint32_t)(q1 & 0xFFFF) << 16);
-              } else {
-                *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + gidx) = make_int2(q0, q1);
-              }
-            }
-          } else if (p.mode == HAWQ_EPI_RESIDUAL) {
-            int32_t r0 = 0, r1 = 0;
-            uint32_t rm0 = p.res_m, rm1 = p.res_m;
-            int re0 = p.res_e, re1 = p.res_e;
-            double rM0 = res_M, rM1 = res_M;
-            uint8_t* rptr = sRes + row * res_pitch + col * res_es;
-            if (res_es == 2) {
-              const uint32_t pr = *reinterpret_cast<const uint32_t*>(rptr);
-              r0 = (int32_t)(pr & 0xFFFFu);
-              r1 = (int32_t)(pr >> 16);
-            } else {
-              const int2 pr = *reinterpret_cast<const int2*>(rptr);
-              r0 = pr.x;
-              r1 = pr.y;
-            }
-            if (p.res_kind == 1) {
-              if constexpr (FAST) {
-                const double2 M1 = *reinterpret_cast<const double2*>(&sM1[col]);
-                rM0 = M1.x; rM1 = M1.y;
-              } else {
-                rm0 = sResChan[col].m; re0 = sResChan[col].e; rm1 = sResChan[col + 1].m; re1 = sResChan[col + 1].e;
-              }
-            }
-            int32_t y0 = sat_add(rq_term(r0, rm0, re0, rM0, ok), rq_term(v0, (uint32_t)c0.y, c0.z, M01.x, ok));
-            int32_t y1 = sat_add(rq_term(r1, rm1, re1, rM1, ok), rq_term(v1, (uint32_t)c1.y, c1.z, M01.y, ok));
-            if (p.relu) { y0 = max(y0, 0); y1 = max(y1, 0); }
-            uint8_t* yptr = sY + row * y_pitch + col * y_es;
-            if (p.y_bits == 32) {
-              if (y_staged) *reinterpret_cast<int2*>(yptr) = make_int2(y0, y1);
-              else if (ok) *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + gidx) = make_int2(y0, y1);
-            } else if (p.y_bits == 16) {
-              if (ok && max(y0, y1) > 65535) atomicOr(p.status, HAWQ_FLAG_RESIDUAL_OVERFLOW);
-              const uint32_t packed = (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
-              if (y_staged) *reinterpret_cast<uint32_t*>(yptr) = packed;
-              else if (ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + gidx) = packed;
-            }
-            if (p.low_bits != 0) {
-              const int32_t q0 = clampi(rq(y0, p.low_m, p.low_e, low_M), p.low_lo, p.low_hi);
-              const int32_t q1 = clampi(rq(y1, p.low_m, p.low_e, low_M), p.low_lo, p.low_hi);
-              *reinterpret_cast<uint16_t*>(sOut + row * S::OUT_PITCH + col) = (uint16_t)((q0 & 0xFF) | ((q1 & 0xFF) << 8));
-            }
-          } else if (p.mode == HAWQ_EPI_RAW_I32) {
-            if (ok) *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + gidx) = make_int2(v0, v1);
-          } else {  // HAWQ_EPI_DEQUANT_F32
-            if (ok) {
-              float* o = reinterpret_cast<float*>(p.out) + (size_t)m * p.cout_store;
-              const int c = n0 + col;
-              if (c < p.cout_store) o[c] = __fmul_rn((float)v0, p.fscale[c]);
-              if (c + 1 < p.cout_store) o[c + 1] = __fmul_rn((float)v1, p.fscale[c + 1]);
-            }
-          }
+        const int m = m0 + warp * 16 + hf * 8 + g;
+        if (m >= p.M) continue;
+        const int32_t v0 = sat_add(acc[ni * 4 + hf * 2 + 0], b0), v1 = sat_add(acc[ni * 4 + hf * 2 + 1], b1);
+        if (p.mode == HAWQ_EPI_RAW_I32) {
+          *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + (size_t)m * p.Cout + n0 + col) = make_int2(v0, v1);
+        } else {
+          float* o = reinterpret_cast<float*>(p.out) + (size_t)m * p.cout_store;
+          const int c = n0 + col;
+          if (c < p.cout_store) o[c] = __fmul_rn((float)v0, p.fscale[c]);
+          if (c + 1 < p.cout_store) o[c + 1] = __fmul_rn((float)v1, p.fscale[c + 1]);
         }
       }
     }
-    if (ovf && p.check_ovf) atomicOr(p.status, HAWQ_FLAG_REQUANT_OVERFLOW);
-  };
-  if (!fast_done) {
-    if (use_slow) epilogue(std::false_type{});
-    else epilogue(std::true_type{});
+  } else {
+    auto run = [&](auto low_out) {
+      if (!fp64) epilogue(RqExact{FAM == FAM_RESIDUAL && p.check_ovf}, low_out);
+      else if (clamped) epilogue(RqFp64<true>{FAM == FAM_RESIDUAL && ratio_over_one}, low_out);
+      else epilogue(RqFp64<false>{FAM == FAM_RESIDUAL && ratio_over_one}, low_out);
+    };
+    if (FAM == FAM_REQUANT && p.out_bits <= 8) run(std::true_type{});
+    else run(std::false_type{});
   }
 
   if (y_staged || stage_low) __syncthreads();
@@ -541,7 +501,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
     }
   }
   if (stage_low) {
-    uint8_t* gout = reinterpret_cast<uint8_t*>(p.mode == HAWQ_EPI_REQUANT ? p.out : p.out_low);
+    uint8_t* gout = reinterpret_cast<uint8_t*>(FAM == FAM_REQUANT ? p.out : p.out_low);
     if (stage_bits == 8) {
       constexpr int CPR = BN / 16;
       for (int id = tid; id < BM * CPR; id += CONV_THREADS) {

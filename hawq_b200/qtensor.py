@@ -32,8 +32,8 @@ class EngineConfig(threading.local):
         HAWQ_FLAG_RESIDUAL_OVERFLOW; ``CompiledModel`` re-runs in 32-bit mode when the flag is raised).
     fast_kernels: False withholds every HAWQ_EP_RATIOS_* promise (always-saturating generic kernels).
     checked: True when the caller reads the device status word after the forward (``CompiledModel`` does).  The plain eager
-        frozen forward does not, so it never promises HAWQ_EP_RATIOS_LE_2P20: the WIDE kernels only *flag* an int32 overflow and
-        rely on the host to re-run, whereas ratios <= 1 cannot overflow and the generic kernels saturate like the reference."""
+        frozen forward does not, so it never promises HAWQ_EP_RATIOS_LE_2P20: the checked FP64 epilogue only *flags* an int32
+        overflow and relies on the host to re-run, whereas ratios <= 1 cannot overflow and the exact form saturates like the reference."""
     residual_bits = 32
     fast_kernels = True
     checked = False

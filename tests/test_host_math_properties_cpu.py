@@ -112,14 +112,15 @@ def bias_window(acc_bound):
 
 
 def fast_signed(v, bias, m, e, acc_bound=ACC_BOUND[8]):
+    """RqFp64 (conv_igemm.cuh): d = v + bias through the folded int -> double conversion (sCb), clamped to int32 in a CTA with a
+    bias outside the window, then one FMA"""
+    d = float(OFF_S + v)                                   # exact: < 2^53
+    cb = float(OFF_S - bias)                               # exact
+    dv = d - cb                                            # exact: v + bias
+    assert Fraction(dv) == v + bias
     lo, hi = bias_window(acc_bound)
-    if lo <= bias <= hi:                                   # bias folded into the int -> double conversion (sCb), not saturated
-        d = float(OFF_S + v)                               # exact: < 2^53
-        cb = float(OFF_S - bias)                           # exact
-        dv = d - cb                                        # exact: v + bias
-        assert Fraction(dv) == v + bias
-    else:                                                  # the CTA takes the sat_add epilogue
-        dv = float(sat32(v + bias))
+    if not lo <= bias <= hi:                               # a clamped CTA
+        dv = min(max(dv, -2.0 ** 31), 2.0 ** 31 - 1)
     y = float(Fraction(dv) * Fraction(m, 2 ** e) + MAGIC)  # the FMA: one rounding
     return _lo_word(y)
 
@@ -153,16 +154,21 @@ def test_fma_requant_is_exact_for_ratios_up_to_one(a_bits, v, bias, m, e):
 
 
 @settings(max_examples=600, deadline=None)
-@given(st.integers(-2 ** 30, 2 ** 30), st.integers(-2 ** 20, 2 ** 20), st.integers(2 ** 30, 2 ** 31), st.integers(11, 40))
+@given(st.integers(-2 ** 30, 2 ** 30), st.integers(-2 ** 31, 2 ** 31 - 1), st.integers(2 ** 30, 2 ** 31), st.integers(11, 40))
+@example(2 ** 30, 2 ** 31 - 1, 2 ** 31, 11)
+@example(-2 ** 30, -2 ** 31, 2 ** 31, 11)
+@example(-2 ** 30, -2 ** 31, 2 ** 30, 40)
+@example(2 ** 30, 2 ** 30, 2 ** 31, 40)
 def test_fma_requant_wide_ratios_with_overflow_check(v, bias, m, e):
-    """ratios up to 2^20: the result is exact whenever the kernel's validity check passes, and the check fails exactly when the
-    rounded value leaves int32 (then HAWQ_FLAG_REQUANT_OVERFLOW is raised and the saturating kernels are used)."""
-    q, hi = fast_signed(v, bias, m, e)
-    exact = Fraction((v + bias) * m, 2 ** e)
+    """ratios up to 2^20, |acc| <= 2^30 and any int32 bias: the result is RHE(sat32(acc + bias) * ratio) whenever the kernel's
+    validity check passes, and the check fails exactly when that rounded value leaves int32 (then HAWQ_FLAG_REQUANT_OVERFLOW is
+    raised and the saturating kernels are used)."""
+    q, hi = fast_signed(v, bias, m, e, acc_bound=2 ** 30)
+    exact = Fraction(sat32(v + bias) * m, 2 ** e)
     fl = math.floor(exact)
     rem = exact - fl
     r = fl + (1 if rem > Fraction(1, 2) or (rem == Fraction(1, 2) and fl % 2 == 1) else 0)   # unsaturated RHE
-    valid = ((hi + ((q >> 31) & 1)) ^ 0x43380000) == 0          # bit-pattern form of the WIDE check in conv_igemm.cuh (t - 1.5 * 2^52 in int32)
+    valid = ((hi + ((q >> 31) & 1)) ^ 0x43380000) == 0          # bit-pattern form of the checked FP64 term in conv_igemm.cuh (t - 1.5 * 2^52 in int32)
     assert valid == (-2 ** 31 <= r < 2 ** 31)
     if valid:
         assert q == r

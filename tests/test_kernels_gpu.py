@@ -622,12 +622,13 @@ def test_stem_pool_declines_shapes_outside_the_kernel(shape):
 
 
 # ------------------------------------------------------------------------------------------------ int32 and ratio boundaries
-# The specialised epilogues of conv_igemm.cuh fold the bias into the int -> double conversion and run one FP64 FMA per term; a CTA
-# leaves them for the saturating or the exact 64-bit epilogue when a bias or a ratio is outside their range.  These tests put
+# Each CTA of conv_igemm.cuh picks its requantisation: FP64 (the bias folded into the int -> double conversion, one FMA per term)
+# when every ratio is <= 1, or for RESIDUAL under a ratio promise when every ratio is <= 2^20 (each term then range-checked); the
+# exact 64-bit form otherwise.  An FP64 CTA with a bias that can take acc + bias out of int32 clamps that sum.  These tests put
 # accumulators, biases and ratios on those limits, side by side with ordinary channels in neighbouring column blocks, and demand
 # whole outputs and the status word equal to the ABI model.
 I32_MIN, I32_MAX = -2 ** 31, 2 ** 31 - 1
-RATIO_ONE = (2 ** 31, 31)           # exactly 1 in the specialised-epilogue form (dyadic(1.0) is (2^30, 30))
+RATIO_ONE = (2 ** 31, 31)           # exactly 1 in the FP64 form (dyadic(1.0) is (2^30, 30))
 WIDE_RATIOS = [dyadic(1.0), dyadic(1 + 2 ** -20), (2 ** 31, 11), dyadic(3.0), dyadic(1000.0)]   # (1, 2^20], 2^20 exactly
 GENERIC_RATIOS = [(2 ** 30 + 1, 10), (2 ** 31, 10), (0, 31), RATIO_ONE]                         # above 2^20, m = 0, 1
 
@@ -657,11 +658,11 @@ def extreme_act(r, n, pix, c, a_bits):
 
 def boundary_weights_chan(r, cout, bn, kh, kw, cin, a_bits):
     """Column block b (BN channels) by b % 4:
-      0: random weights, |bias| <= 2^16, ratios <= 1 (0.5 and 0.25 give round-half-even ties): the specialised epilogue;
+      0: random weights, |bias| <= 2^16, ratios <= 1 (0.5 and 0.25 give round-half-even ties): FP64;
       1: bias edges (int32 limits, both sides of the bias window, 0) on constant weight rows -128 / 127 / -127 and random rows,
          ratios <= 1 (1 exactly, 5e-8, m = 0, log-uniform down to 1e-9);
-      2: as 1, plus zero-weight channels with a small bias and a ratio in (1, 2^20] (the checked wide epilogue's range);
-      3: as 0, plus zero-weight channels with a small bias and a ratio above 2^20, m = 0 or exactly 1 (the exact 64-bit epilogue).
+      2: as 1, plus zero-weight channels with a small bias and a ratio in (1, 2^20] (FP64, clamped and checked, under a promise);
+      3: as 0, plus zero-weight channels with a small bias and a ratio above 2^20, m = 0 or exactly 1 (the exact 64-bit form).
     Zero-weight channels keep |bias| <= 1000, so that no term leaves int32 at ratios up to 2^21."""
     k = kh * kw * cin
     edges = edge_biases(k, a_bits)
@@ -705,7 +706,7 @@ BOUNDARY_GEOMS = [
     (3, 9, 9, 128, 512, 1, 1, 1, 0),      # 1x1, M = 243: two row tiles
 ]
 REQUANT_CASES = [(out_bits, clamp, relu) for out_bits, clamp in [(4, (0, 15)), (8, (-128, 127)), (16, (-32768, 32767)), (32, (I32_MIN, I32_MAX))]
-                 for relu in (0, 1)]
+                 for relu in (0, 1)] + [(8, (-128, -5), 1)]   # ReLU with clamp_hi < 0: every output is clamp_hi
 RESIDUAL_CASES = [  # res_kind, res_bits, y_bits, low_bits, relu
     (0, 16, 16, 8, 1), (0, 32, 32, 4, 1), (0, 32, 32, 0, 0), (0, 16, 0, 4, 1), (1, 32, 16, 4, 1), (1, 32, 0, 8, 1), (1, 32, 32, 0, 0)]
 
@@ -737,7 +738,7 @@ def test_conv_epilogue_boundaries(geom, a_bits, flags):
                 failed.append((what, k_, int((a != b).sum())))
 
     for out_bits, clamp, relu in REQUANT_CASES:
-        check(ops.epilogue(EPI_REQUANT, relu=relu, out_bits=out_bits, clamp=clamp, flags=flags), ("requant", out_bits, relu),
+        check(ops.epilogue(EPI_REQUANT, relu=relu, out_bits=out_bits, clamp=clamp, flags=flags), ("requant", out_bits, clamp, relu),
               out=out_buf(numel, out_bits))
     res_chan = res_chan_with_ties(r, cout)
     for res_kind, res_bits, y_bits, low_bits, relu in RESIDUAL_CASES:
