@@ -171,6 +171,8 @@ int hawq_stem_pool_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int
                       int32_t clamp_lo, int32_t clamp_hi, int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
                       int32_t low_lo, int32_t low_hi, void* out_low, void* stream);
 /* nn.MaxPool2d(3,2,1) (q_resnet.py:119) on the int16 stem output + the first unit's quant_act (case 0, scalar m,e).
+ * Precondition: 0 <= x <= 32767 (the post-ReLU stem output); the kernel pads with 0 and reads the maxima as unsigned, so
+ * negative inputs give unspecified results.
  * y: residual stream (y_bits 16 -> uint16, 32 -> int32); out_low: int8 / packed u4 (low_bits 8 / 4, 0 = none). */
 int hawq_maxpool_requant(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_t C, const int16_t* x,
                          int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
@@ -183,7 +185,8 @@ int hawq_avgpool_requant(hawq_handle* h, int32_t N, int32_t HW, int32_t C, int32
 
 /* ---- stand-alone (unfused) pieces of the module API --------------------------------------------------------- */
 /* QuantAct input branch (quant_modules.py:271-274): q = clamp(round((1/scale) * x)), fp32 RNE.
- * x fp32 NCHW [N,C,H,W] -> int8 NHWC [N,H,W,C]. */
+ * x fp32 NCHW [N,C,H,W] -> int8 NHWC [N,H,W,C].  +-inf clamp to lo / hi.  NaN is outside the reference's semantics (its
+ * integer cast of NaN is undefined): the result for a NaN element is unspecified. */
 int hawq_quantize_input_f32(hawq_handle* h, int32_t N, int32_t C, int32_t H, int32_t W, const float* x,
                             float scale, int32_t lo, int32_t hi, int8_t* out, void* stream);
 /* uint8 image entry (tvm_benchmark/test_resnet_accuracy_imagenet.py:62-75 quantize_image after transforms.ToTensor + Normalize

@@ -162,6 +162,7 @@ def stem_pool(x, w256, chan, clamp, n, hh, ww, y_bits, y, low_bits, low_me, low_
 
 def maxpool_requant(x, n, hh, ww, c, y_bits, y, low_bits, low_me, low_clamp, out_low):
     xa = decode(x, 16, True).reshape(n, hh, ww, c)
+    assert xa.min(initial=0) >= 0, "hawq_maxpool_requant needs x >= 0 (it pads with 0 and reads the maxima as unsigned)"
     p = ir.maxpool_3x3_s2_p1(xa)
     if y_bits:
         encode_into(y, p, y_bits)
