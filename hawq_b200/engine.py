@@ -188,24 +188,26 @@ class CompiledModel:
             out = self.outs[self.residual_bits]
             if post is not None:
                 out = post(out)
+            # three host logits buffers: batch i's is yielded during iteration i + 1 and must survive iteration i + 2, which
+            # already enqueues the read-back of batch i + 2
             self._pipe = dict(copy=cs, stage=[torch.empty_like(self.static_in) for _ in range(2)],
-                              out=[torch.empty(out.shape, dtype=out.dtype).pin_memory() for _ in range(2)],
+                              out=[torch.empty(out.shape, dtype=out.dtype).pin_memory() for _ in range(3)],
                               flag=[torch.zeros(self.all_flags.numel() if self.gather else 1, dtype=torch.int32).pin_memory() for _ in range(2)],
                               h2d=[torch.cuda.Event() for _ in range(2)], free=[torch.cuda.Event() for _ in range(2)],
                               done=[torch.cuda.Event() for _ in range(2)])
         P = self._pipe
         prev = None
 
-        def finish(slot, xb):
+        def finish(slot, oslot, xb):
             P["done"][slot].synchronize()
             if self._flags(P["flag"][slot].tolist()) & 7:
                 self(xb)                            # rare: exact fallback path, synchronous (sharded runs: every rank takes it together)
                 out = self.outs[self._last_key]
                 return (post(out) if post is not None else out).to("cpu")
-            return P["out"][slot]
+            return P["out"][oslot]
 
         for i, xb in enumerate(host_batches):
-            slot = i & 1
+            slot, oslot = i & 1, i % 3
             with torch.cuda.stream(P["copy"]):
                 P["copy"].wait_event(P["free"][slot])
                 P["stage"][slot].copy_(xb, non_blocking=True)
@@ -216,12 +218,12 @@ class CompiledModel:
             out = self._run(self.residual_bits)
             if post is not None:
                 out = post(out)
-            P["out"][slot].copy_(out, non_blocking=True)
+            P["out"][oslot].copy_(out, non_blocking=True)
             P["flag"][slot].copy_(self.all_flags if self.gather else self.flag, non_blocking=True)
             P["done"][slot].record(main)
             if prev is not None:
                 yield finish(*prev)
-            prev = (slot, xb)
+            prev = (slot, oslot, xb)
         if prev is not None:
             yield finish(*prev)
 

@@ -28,6 +28,10 @@ CALIB_BATCH, CALIB_SEED = 4, 0
 PARITY_BATCH, PARITY_SEED = 2, 1
 NET_CONFIGS = [("resnet18", "uniform8"), ("resnet18", "uniform4"), ("resnet18", "bops_0.5"),
                ("resnet50", "uniform8"), ("resnet50", "uniform4"), ("resnet50", "bops_0.5")]
+# the published HAWQ-V3 mixed-precision tables (ResNet-18 latency_0.75 / latency_0.25 equal bops_0.75 / bops_0.25)
+NET_CONFIGS += [("resnet18", s) for s in ("modelsize_0.75", "modelsize_0.5", "modelsize_0.25", "bops_0.75", "bops_0.25", "latency_0.5")]
+NET_CONFIGS += [("resnet50", s) for s in ("modelsize_0.75", "modelsize_0.5", "modelsize_0.25", "bops_0.75", "bops_0.25",
+                                          "latency_0.75", "latency_0.5", "latency_0.25")]
 
 
 def sha_i32(a):

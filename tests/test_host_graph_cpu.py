@@ -11,7 +11,7 @@ from hawq_b200.build import build_library
 from hawq_b200.synthetic import synthetic_batch
 from oracle import int_ref as ir
 from tests import abi_model
-from tests.util import build_fakequant, golden_act_ranges, load_net_golden, sha_i32
+from tests.util import RESNET_GOLDENS, build_fakequant, golden_act_ranges, load_net_golden, sha_i32
 
 
 @pytest.fixture(scope="session", autouse=True)
@@ -28,11 +28,11 @@ def _hook_outputs(q):
     return rec, hooks
 
 
-@pytest.mark.parametrize("arch,scheme,res_bits,a4_container", [("resnet18", "uniform8", 32, 8), ("resnet18", "uniform4", 16, 8),
-                                                               ("resnet18", "uniform4", 32, 4), ("resnet18", "bops_0.5", 32, 8),
-                                                               ("resnet50", "bops_0.5", 16, 4), ("resnet101", "uniform4", 16, 8)])
+@pytest.mark.parametrize("arch,scheme,res_bits,a4_container",
+                         [(a, s) + ((16, 8) if i % 2 == 0 else (32, 4)) for i, (a, s) in enumerate(RESNET_GOLDENS)])
 def test_frozen_graph_matches_golden(monkeypatch, arch, scheme, res_bits, a4_container):
-    """a4_container: 4-bit activations stored one per byte (default) or as packed nibbles - same integers either way."""
+    """a4_container: 4-bit activations stored one per byte (default) or as packed nibbles - same integers either way.  The
+    goldens alternate between the uint16 stream with byte containers and the int32 stream with packed nibbles."""
     abi_model.install_cpu_backend(monkeypatch)
     monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
     logits_g, meta = load_net_golden(arch, scheme)

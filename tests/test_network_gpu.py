@@ -8,19 +8,23 @@ import hawq_b200 as hb
 from hawq_b200 import qtensor
 from hawq_b200.synthetic import synthetic_batch
 from oracle import int_ref as ir
-from tests.util import build_fakequant, golden_act_ranges, load_net_golden, sha_i32
+from tests.util import RESNET_GOLDENS, build_fakequant, golden_act_ranges, load_net_golden, sha_i32
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-CONFIGS = [("resnet18", "uniform8"), ("resnet18", "uniform4"), ("resnet18", "bops_0.5"),
-           ("resnet50", "uniform8"), ("resnet50", "uniform4"), ("resnet50", "bops_0.5"), ("resnet101", "uniform8")]
+# every golden at a4_container 8, and packed nibbles too for the schemes with 4-bit activations
+A4_CONFIGS = [(a, s, 8) for a, s in RESNET_GOLDENS] + [(a, s, 4) for a, s in RESNET_GOLDENS
+                                                       if any(v["bits"] == 4 for v in load_net_golden(a, s)[1]["acts"].values())]
+# resize units whose identity input is 4-bit and whose last convolution's input is 8-bit: with packed nibbles the two 1x1 inputs
+# have different widths, so the dual kernel is declined there (identity RAW_I32 conv + RESIDUAL conv instead)
+MIXED_WIDTH_RESIZE = {("resnet50", "modelsize_0.25"): 1, ("resnet50", "latency_0.25"): 1}
 
 
 def _model(arch, scheme, meta):
     return hb.build_synthetic_qresnet(arch, scheme, act_ranges=golden_act_ranges(meta))
 
 
-@pytest.mark.parametrize("arch,scheme", CONFIGS)
+@pytest.mark.parametrize("arch,scheme", RESNET_GOLDENS)
 @pytest.mark.parametrize("res_bits", [32, 16])
 def test_eager_module_api_matches_golden(arch, scheme, res_bits):
     """Frozen module-by-module forward (the drop-in API) on fp32 NCHW CUDA input: logits bit-equal to the reference."""
@@ -38,7 +42,7 @@ def test_eager_module_api_matches_golden(arch, scheme, res_bits):
     assert np.array_equal(out.cpu().numpy(), logits_g)
 
 
-@pytest.mark.parametrize("arch,scheme", [("resnet18", "uniform4"), ("resnet50", "bops_0.5")])
+@pytest.mark.parametrize("arch,scheme", RESNET_GOLDENS)
 def test_every_activation_matches_oracle(arch, scheme):
     """Mirror of the reference's --debug-unit checks: integer equality at every QuantAct / unit boundary."""
     logits_g, meta = load_net_golden(arch, scheme)
@@ -69,13 +73,12 @@ def test_every_activation_matches_oracle(arch, scheme):
     assert np.array_equal(out.cpu().numpy(), logits_g)
 
 
-@pytest.mark.parametrize("arch,scheme,a4_container", [("resnet18", "uniform8", 8), ("resnet50", "uniform8", 8), ("resnet50", "uniform4", 8),
-                                                      ("resnet50", "uniform4", 4), ("resnet50", "bops_0.5", 8), ("resnet50", "bops_0.5", 4),
-                                                      ("resnet18", "uniform4", 4)])
+@pytest.mark.parametrize("arch,scheme,a4_container", A4_CONFIGS)
 def test_compiled_graph_int8_input_and_batch_invariance(arch, scheme, a4_container, monkeypatch):
     """CUDA-graph engine on int8 NHWC input at a larger batch: the first two images are the golden inputs, so their
     logits must equal the golden logits whatever else is in the batch (size-independent property); replays are idempotent.
-    a4_container: 4-bit activations one per byte (default) or as packed nibbles expanded on chip - same logits."""
+    a4_container: 4-bit activations one per byte (default) or as packed nibbles expanded on chip - same logits.
+    The uint16 stream runs each bottleneck resize unit as one dual kernel, except where the two inputs differ in width."""
     monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
     logits_g, meta = load_net_golden(arch, scheme)
     q = _model(arch, scheme, meta)
@@ -91,6 +94,15 @@ def test_compiled_graph_int8_input_and_batch_invariance(arch, scheme, a4_contain
     assert torch.equal(out1, out2)
     assert np.array_equal(out1[:2].cpu().numpy(), logits_g)
     assert eng.gpu_launches > 0
+    # one eager checked forward at residual_bits = 16: one dual kernel per bottleneck resize unit of equal input widths
+    duals = 0 if arch == "resnet18" else 4 - (MIXED_WIDTH_RESIZE.get((arch, scheme), 0) if a4_container == 4 else 0)
+    n, h, w, c = q_in.shape
+    before = hb._lib.load().hawq_debug_kernel_count(4)
+    with torch.no_grad(), qtensor.engine_mode(residual_bits=16, checked=True):
+        out_e = q(hb.IntActivation(qtensor.Node("int", (n, c, h, w), data=q_in.view(-1), bits=8, signed=True), q_in.device))
+    torch.cuda.synchronize()
+    assert hb._lib.load().hawq_debug_kernel_count(4) - before == duals
+    assert torch.equal(out_e, out1)
     # exactness fallback: int32 residual graph gives the same logits
     eng32 = hb.compile_model(q, q_in, residual_bits=32)
     assert torch.equal(eng32(q_in), out1)

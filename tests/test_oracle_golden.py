@@ -8,7 +8,7 @@ import torch
 
 from oracle import fakequant as fq
 from oracle import int_ref as ir
-from tests.util import load_golden, load_net_golden, sha_i32, build_fakequant
+from tests.util import RESNET_GOLDENS, load_golden, load_net_golden, sha_i32, build_fakequant
 from hawq_b200.synthetic import synthetic_batch
 
 
@@ -112,8 +112,7 @@ def test_module_kats():
     assert np.array_equal(q, g["pool_q"].transpose(0, 2, 3, 1))
 
 
-@pytest.mark.parametrize("arch,scheme", [("resnet18", "uniform8"), ("resnet18", "uniform4"), ("resnet18", "bops_0.5"),
-                                         ("resnet50", "bops_0.5"), ("resnet101", "uniform8")])
+@pytest.mark.parametrize("arch,scheme", RESNET_GOLDENS)
 def test_network_golden(arch, scheme):
     """Whole network: fakequant and int_ref reproduce the reference's activation integers (sha256 over every
     QuantAct output), integer weights and bit-equal logits."""

@@ -7,6 +7,9 @@ import numpy as np
 import torch
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+# (arch, scheme) of every ResNet network golden (net_<arch>_<scheme>.npz, written by tests/golden/make_golden.py)
+RESNET_GOLDENS = sorted(tuple(f[len("net_"):-len(".npz")].split("_", 1)) for f in os.listdir(GOLDEN)
+                        if f.startswith("net_resnet") and f.endswith(".npz"))
 
 
 def load_golden(name):
