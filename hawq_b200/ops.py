@@ -40,21 +40,22 @@ def _p(t):
 timer = None   # set to a list to record (kernel, info, start_event, end_event) per launch (bench.py roofline leg)
 
 
-def _begin():
-    if timer is None:
-        return None
-    ev = torch.cuda.Event(enable_timing=True)
-    ev.record()
-    return ev
-
-
-def _count(name="", info=None, ev0=None):
+def _launch(t, fn, *args, label=None, work=None):
+    """Calls ABI entry point `fn`(handle, *args, stream) on the device and current stream of tensor `t` and counts the launch.
+    While `timer` is set, a launch with a `label` is bracketed by CUDA events and recorded with `work()`, its (MACs, bytes)."""
     global launch_count
+    h, s = _ctx(t)
+    ev0 = None
+    if label is not None and timer is not None:
+        ev0 = torch.cuda.Event(enable_timing=True)
+        ev0.record()
+    _lib.check(getattr(_lib.load(), fn)(h, *args, s))
     launch_count += 1
     if ev0 is not None:
+        info = work()
         ev1 = torch.cuda.Event(enable_timing=True)
         ev1.record()
-        timer.append((name, info, ev0, ev1))
+        timer.append((label, info, ev0, ev1))
 
 
 def conv_work(desc, ep):
@@ -132,82 +133,59 @@ def ratio_flags(*pairs):
 
 
 def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None, out_low=None):
-    h, s = _ctx(x)
-    ev = _begin()
-    lib = _lib.load()
-    _lib.check(lib.hawq_conv2d(h, C.byref(desc), C.byref(ep), _p(x), _p(w), _p(chan), _p(res), _p(res_chan),
-                               _p(fscale), _p(out), _p(out_low), s))
-    if ev is not None:     # per-launch timing (bench.py roofline leg)
-        _count("conv_igemm", conv_work(desc, ep), ev)
-    else:
-        _count()
+    _launch(x, "hawq_conv2d", C.byref(desc), C.byref(ep), _p(x), _p(w), _p(chan), _p(res), _p(res_chan), _p(fscale), _p(out),
+            _p(out_low), label="conv_igemm", work=lambda: conv_work(desc, ep))
 
 
 def conv2d_dual(x, desc, ep, w, chan, desc2, x2, w2, chan2, out=None, out_low=None):
     """resize unit: identity 1x1 conv (desc2/x2/w2/chan2) + last 1x1 conv (desc/x/w/chan) + case-1 sum in one kernel."""
-    h, s = _ctx(x)
-    ev = _begin()
-    _lib.check(_lib.load().hawq_conv2d_dual(h, C.byref(desc), C.byref(ep), _p(x), _p(w), _p(chan), C.byref(desc2), _p(x2), _p(w2),
-                                            _p(chan2), _p(out), _p(out_low), s))
-    work = None
-    if ev is not None:
+    def work():
         m = desc.N * desc.H * desc.W
         macs = m * desc.Cout * (desc.Cin + desc2.Cin)
         b = (m * (desc.Cin + desc2.Cin) * desc.a_bits // 8 + desc.Cout * (desc.Cin + desc2.Cin) + 32 * desc.Cout
              + m * desc.Cout * (ep.y_bits + ep.low_bits) // 8)
-        work = (macs, b)
-    _count("conv_dual", work, ev)
+        return macs, b
+    _launch(x, "hawq_conv2d_dual", C.byref(desc), C.byref(ep), _p(x), _p(w), _p(chan), C.byref(desc2), _p(x2), _p(w2), _p(chan2),
+            _p(out), _p(out_low), label="conv_dual", work=work)
 
 
 def linear(x, w, chan, fscale, out, n, k, cout, cout_pad):
-    h, s = _ctx(x)
-    ev = _begin()
-    _lib.check(_lib.load().hawq_linear_i8(h, n, k, cout, cout_pad, _p(x), _p(w), _p(chan), _p(fscale), _p(out), s))
-    _count("hawq_linear", (n * k * cout, n * k + cout_pad * k + 20 * cout_pad + n * cout * 4) if ev is not None else None, ev)
+    _launch(x, "hawq_linear_i8", n, k, cout, cout_pad, _p(x), _p(w), _p(chan), _p(fscale), _p(out), label="hawq_linear",
+            work=lambda: (n * k * cout, n * k + cout_pad * k + 20 * cout_pad + n * cout * 4))
 
 
 def stem_conv(x, w, chan, clamp, out, n, hh, ww):
-    h, s = _ctx(x)
-    ev = _begin()
-    _lib.check(_lib.load().hawq_stem_conv_i8(h, n, hh, ww, _p(x), _p(w), _p(chan), clamp[0], clamp[1], _p(out), s))
     ho, wo = (hh - 1) // 2 + 1, (ww - 1) // 2 + 1
-    _count("stem_conv", (n * ho * wo * 64 * 147, n * hh * ww * 3 + 64 * 224 + 1024 + n * ho * wo * 64 * 2) if ev is not None else None, ev)
+    _launch(x, "hawq_stem_conv_i8", n, hh, ww, _p(x), _p(w), _p(chan), clamp[0], clamp[1], _p(out), label="stem_conv",
+            work=lambda: (n * ho * wo * 64 * 147, n * hh * ww * 3 + 64 * 224 + 1024 + n * ho * wo * 64 * 2))
 
 
 def stem_pool(x, w256, chan, clamp, n, hh, ww, y_bits, y, low_bits, low_me, low_clamp, out_low):
     """Fused stem (conv 7x7/2 + max-pool 3x3/2 + 16-bit requant + ReLU + low-bit copy) in one kernel; raises HawqError(ERR_UNSUPPORTED)
     for shapes / ratios outside it (callers then use stem_conv + maxpool_requant, same integers)."""
-    h, s = _ctx(x)
-    ev = _begin()
-    _lib.check(_lib.load().hawq_stem_pool_i8(h, n, hh, ww, _p(x), _p(w256), _p(chan), clamp[0], clamp[1], y_bits, _p(y), low_bits, low_me[0],
-                                             low_me[1], low_clamp[0], low_clamp[1], _p(out_low), s))
     ho, wo = (hh - 1) // 2 + 1, (ww - 1) // 2 + 1
     po, qo = (ho - 1) // 2 + 1, (wo - 1) // 2 + 1
-    _count("stem_pool", (n * ho * wo * 64 * 147, n * hh * ww * 3 + 64 * 256 + 1024 + n * po * qo * 64 * (y_bits + low_bits) // 8) if ev is not None else None, ev)
+    _launch(x, "hawq_stem_pool_i8", n, hh, ww, _p(x), _p(w256), _p(chan), clamp[0], clamp[1], y_bits, _p(y), low_bits, low_me[0],
+            low_me[1], low_clamp[0], low_clamp[1], _p(out_low), label="stem_pool",
+            work=lambda: (n * ho * wo * 64 * 147, n * hh * ww * 3 + 64 * 256 + 1024 + n * po * qo * 64 * (y_bits + low_bits) // 8))
 
 
 def maxpool_requant(x, n, hh, ww, c, y_bits, y, low_bits, low_me, low_clamp, out_low):
-    h, s = _ctx(x)
-    ev = _begin()
-    _lib.check(_lib.load().hawq_maxpool_requant(h, n, hh, ww, c, _p(x), y_bits, _p(y), low_bits, low_me[0], low_me[1],
-                                                low_clamp[0], low_clamp[1], _p(out_low), s))
     po, qo = (hh - 1) // 2 + 1, (ww - 1) // 2 + 1
-    _count("maxpool_requant", (0, n * hh * ww * c * 2 + n * po * qo * c * (y_bits + low_bits) // 8) if ev is not None else None, ev)
+    _launch(x, "hawq_maxpool_requant", n, hh, ww, c, _p(x), y_bits, _p(y), low_bits, low_me[0], low_me[1], low_clamp[0],
+            low_clamp[1], _p(out_low), label="maxpool_requant",
+            work=lambda: (0, n * hh * ww * c * 2 + n * po * qo * c * (y_bits + low_bits) // 8))
 
 
 def avgpool_requant(x, n, hw, c, x_bits, me, clamp, out):
-    h, s = _ctx(x)
-    ev = _begin()
-    _lib.check(_lib.load().hawq_avgpool_requant(h, n, hw, c, x_bits, _p(x), me[0], me[1], clamp[0], clamp[1], _p(out), s))
-    _count("avgpool_requant", (0, n * hw * c * x_bits // 8 + n * c) if ev is not None else None, ev)
+    _launch(x, "hawq_avgpool_requant", n, hw, c, x_bits, _p(x), me[0], me[1], clamp[0], clamp[1], _p(out), label="avgpool_requant",
+            work=lambda: (0, n * hw * c * x_bits // 8 + n * c))
 
 
 def quantize_input(x, scale, clamp, out):
     n, c, hh, ww = x.shape
-    h, s = _ctx(x)
-    ev = _begin()
-    _lib.check(_lib.load().hawq_quantize_input_f32(h, n, c, hh, ww, _p(x), float(scale), clamp[0], clamp[1], _p(out), s))
-    _count("quantize_input", (0, n * c * hh * ww * 5) if ev is not None else None, ev)
+    _launch(x, "hawq_quantize_input_f32", n, c, hh, ww, _p(x), float(scale), clamp[0], clamp[1], _p(out), label="quantize_input",
+            work=lambda: (0, n * c * hh * ww * 5))
 
 
 def quantize_input_u8(x, mean, std, scale, clamp, out):
@@ -215,43 +193,29 @@ def quantize_input_u8(x, mean, std, scale, clamp, out):
     n, hh, ww, c = x.shape
     if c != 3:
         raise ValueError("quantize_input_u8 expects NHWC images with 3 channels")
-    h, s = _ctx(x)
-    ev = _begin()
     m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
-    _lib.check(_lib.load().hawq_quantize_input_u8(h, n, hh, ww, _p(x), m3, s3, float(scale), clamp[0], clamp[1], _p(out), s))
-    _count("quantize_input_u8", (0, n * hh * ww * 6) if ev is not None else None, ev)
+    _launch(x, "hawq_quantize_input_u8", n, hh, ww, _p(x), m3, s3, float(scale), clamp[0], clamp[1], _p(out),
+            label="quantize_input_u8", work=lambda: (0, n * hh * ww * 6))
 
 
 def requant(x, rows, c, x_bits, chan, chan_stride, relu, out_bits, clamp, out):
-    h, s = _ctx(x)
-    _lib.check(_lib.load().hawq_requant(h, rows, c, x_bits, _p(x), _p(chan), chan_stride, int(relu), out_bits,
-                                        clamp[0], clamp[1], _p(out), s))
-    _count()
+    _launch(x, "hawq_requant", rows, c, x_bits, _p(x), _p(chan), chan_stride, int(relu), out_bits, clamp[0], clamp[1], _p(out))
 
 
 def add_requant(acc, rows, c, chan, ep, res, res_chan, y, out_low):
-    h, s = _ctx(acc)
-    _lib.check(_lib.load().hawq_add_requant(h, rows, c, _p(acc), _p(chan), C.byref(ep), _p(res), _p(res_chan), _p(y),
-                                            _p(out_low), s))
-    _count()
+    _launch(acc, "hawq_add_requant", rows, c, _p(acc), _p(chan), C.byref(ep), _p(res), _p(res_chan), _p(y), _p(out_low))
 
 
 def dequant(x, n, hh, ww, c, x_bits, x_signed, scale, out):
-    h, s = _ctx(x)
-    _lib.check(_lib.load().hawq_dequant_f32(h, n, hh, ww, c, x_bits, int(x_signed), _p(x), float(scale), _p(out), s))
-    _count()
+    _launch(x, "hawq_dequant_f32", n, hh, ww, c, x_bits, int(x_signed), _p(x), float(scale), _p(out))
 
 
 def pack_i4(src, dst):
-    h, s = _ctx(src)
-    _lib.check(_lib.load().hawq_pack_i4(h, src.numel(), _p(src), _p(dst), s))
-    _count()
+    _launch(src, "hawq_pack_i4", src.numel(), _p(src), _p(dst))
 
 
 def unpack_i4(src, dst):
-    h, s = _ctx(src)
-    _lib.check(_lib.load().hawq_unpack_i4(h, dst.numel(), _p(src), _p(dst), s))
-    _count()
+    _launch(src, "hawq_unpack_i4", dst.numel(), _p(src), _p(dst))
 
 
 def reset_status(device_index):

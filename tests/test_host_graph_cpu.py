@@ -6,7 +6,7 @@ import pytest
 import torch
 
 import hawq_b200 as hb
-from hawq_b200 import qtensor
+from hawq_b200 import ops, qtensor
 from hawq_b200.build import build_library
 from hawq_b200.synthetic import synthetic_batch
 from oracle import int_ref as ir
@@ -73,6 +73,15 @@ def test_frozen_graph_matches_golden(monkeypatch, arch, scheme, res_bits, a4_con
     assert checked >= len(meta["acts"]) - 2
     for h in hooks:
         h.remove()
+    if res_bits == 16:
+        # the mode CompiledModel runs: checked, so the 4-bit schemes may promise ratios <= 2^20 too.  Every bottleneck resize
+        # unit takes the dual kernel; ResNet-18's resize units are 3x3 and never do
+        duals = []
+        monkeypatch.setattr(ops, "conv2d_dual", lambda *a, **kw: (duals.append(a), abi_model.conv2d_dual(*a, **kw)))
+        with torch.no_grad(), qtensor.engine_mode(residual_bits=16, checked=True):
+            out = q(x)
+        assert np.array_equal(out.numpy(), logits_g)
+        assert len(duals) == (0 if arch == "resnet18" else 4)
 
 
 def test_frozen_requires_cuda():
