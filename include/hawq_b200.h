@@ -10,6 +10,11 @@
  *   - every call is asynchronous on the caller-supplied stream (cudaStream_t passed as void*), never allocates,
  *     never synchronises -> safe under CUDA-graph capture;
  *   - return value: 0 = HAWQ_OK, negative = hawq_status; hawq_last_error() gives a thread-local message;
+ *   - every device pointer must be 16-byte aligned (the kernels move activations, weights and outputs in 16-byte vectors);
+ *   - a call writes exactly the elements of its outputs and nothing else: a packed 4-bit output is numel / 2 bytes, DEQUANT_F32
+ *     writes rows of cout_store floats, hawq_linear_i8 writes N x Cout floats.  It never writes its inputs, and it neither reads
+ *     nor writes a pointer its arguments leave unused (res / res_chan / fscale / out_low of an epilogue that does not take them,
+ *     out with y_bits 0, out_low with low_bits 0), so such a pointer may be null or point anywhere;
  *   - activations are NHWC.  8-bit: one int8 per element.  4-bit: unsigned nibbles packed two per byte in the
  *     "hawq nibble order": inside every group of 8 consecutive channels, byte j (0..3) holds channel j in its low
  *     nibble and channel j+4 in its high nibble (so a 32-bit word expands to two int8x4 words with one AND and one

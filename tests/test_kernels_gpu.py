@@ -5,8 +5,9 @@ import pytest
 import torch
 
 from hawq_b200 import ops
-from hawq_b200._lib import EPI_DEQUANT_F32, EPI_RAW_I32, EPI_REQUANT, EPI_RESIDUAL, HawqError, dyadic
+from hawq_b200._lib import EPI_DEQUANT_F32, EPI_RAW_I32, EPI_REQUANT, EPI_RESIDUAL, HawqError, dyadic, hawq_conv_desc
 from tests import abi_model as am
+from tests.util import POISON, guarded_call
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -38,18 +39,25 @@ def out_buf(numel, bits):
     return torch.zeros(numel // 2 if bits == 4 else numel, dtype=dt)
 
 
+def widest_row_bytes(args):
+    """bytes of the widest row a call touches, at 4 bytes per element: a convolution row is Cin or Cout channels"""
+    dims = [v for d in args.values() if isinstance(d, hawq_conv_desc) for v in (d.Cin, d.Cout)]
+    return 4 * max(dims + [args[k] for k in ("c", "k", "cout_pad") if k in args] + [64])
+
+
 def run_both(fn_name, cpu_args, out_keys, gpu_overrides=None):
     """cpu_args: dict of kwargs with CPU tensors; out_keys: names of output tensors.  Returns (cpu_outs, gpu_outs).
-    Both status words start at 0, and the library's must equal the model's after the call."""
-    gpu_args = {k: (v.to(DEV) if torch.is_tensor(v) else v) for k, v in cpu_args.items()}
-    gpu_args.update(gpu_overrides or {})
+    The model runs first.  The library then runs with every tensor in a guarded, poisoned allocation (tests/util.guarded_call):
+    its outputs must equal the model's byte for byte, every output byte must be written, and no guard byte, input or unused
+    buffer may change.  Both status words start at 0, and the library's must equal the model's after the call."""
     ops.reset_status(0)
     am.status["flags"] = 0
     getattr(am, fn_name)(**cpu_args)
-    getattr(ops, fn_name)(**gpu_args)
-    torch.cuda.synchronize()
+    args = dict(cpu_args, **(gpu_overrides or {}))
+    outs, problems = guarded_call(getattr(ops, fn_name), args, {k: cpu_args[k] for k in out_keys}, DEV, 128 * widest_row_bytes(args))
     assert ops.get_status(0) == am.status["flags"], (fn_name, ops.get_status(0), am.status["flags"])
-    return [cpu_args[k] for k in out_keys], [gpu_args[k].cpu() for k in out_keys]
+    assert not problems, (fn_name, problems)
+    return [cpu_args[k] for k in out_keys], [outs[k].cpu() for k in out_keys]
 
 
 CONV_GEOMS = [
@@ -319,6 +327,105 @@ def test_conv_raw_and_dequant():
     fs = torch.from_numpy(r.uniform(1e-5, 1e-3, size=cp).astype(np.float32))
     (c,), (g,) = run_both("linear", dict(x=xl, w=wl, chan=chl, fscale=fs, out=torch.zeros((nb, co)), n=nb, k=kk, cout=co, cout_pad=cp), ["out"])
     assert torch.equal(c, g)
+
+
+@pytest.mark.parametrize("a_bits", [8, 4])
+@pytest.mark.parametrize("geom", [CONV_GEOMS[1], CONV_GEOMS[2], CONV_GEOMS[4]])
+def test_conv_raw_and_dequant_geoms(geom, a_bits):
+    """RAW_I32, and DEQUANT_F32 with an odd cout_store below Cout (rows of cout_store floats; the last column block is stored in
+    part), over ragged 3x3, strided and BN = 64 geometries with 8- and 4-bit inputs."""
+    n, h, w, cin, cout, kh, kw, s, p = geom
+    r = rng(1303 + sum(v * (i + 3) for i, v in enumerate(geom)) * 8 + a_bits)
+    ho, wo = out_hw(h, w, kh, kw, s, p)
+    m = n * ho * wo
+    x = rand_act(r, n * h * w * cin, a_bits)
+    wt = torch.from_numpy(r.randint(-128, 128, size=(cout, kh, kw, cin)).astype(np.int8))
+    if a_bits == 4:
+        ops.permute_weights_for_i4(wt)
+    chan = make_chan(r, cout, bias_mag=2 ** 20)
+    d = ops.conv_desc(n, h, w, cin, cout, kh, kw, s, p, a_bits)
+    (c,), (g,) = run_both("conv2d", dict(x=x, desc=d, ep=ops.epilogue(EPI_RAW_I32, flags=TC_FLAG), w=wt, chan=chan, out=out_buf(m * cout, 32)),
+                          ["out"])
+    assert torch.equal(c, g), (geom, a_bits)
+    cs = cout - 63
+    fs = torch.from_numpy(r.uniform(1e-5, 1e-3, size=cout).astype(np.float32))
+    (c,), (g,) = run_both("conv2d", dict(x=x, desc=d, ep=ops.epilogue(EPI_DEQUANT_F32, cout_store=cs), w=wt, chan=chan, fscale=fs,
+                                         out=torch.zeros(m * cs)), ["out"])
+    assert torch.equal(c.view(torch.int32), g.view(torch.int32)), (geom, a_bits)
+
+
+def poisoned(numel, dtype):
+    """a buffer the call must ignore: every byte POISON"""
+    return torch.full((numel * torch.empty(0, dtype=dtype).element_size(),), POISON, dtype=torch.uint8).view(dtype)
+
+
+def test_unused_pointers_stay_untouched():
+    """Every pointer a descriptor leaves unused is passed non-null and poisoned (run_both requires it to stay byte-identical):
+    res / res_chan / out_low of REQUANT, RAW_I32 and DEQUANT_F32, fscale outside DEQUANT_F32, out with y_bits 0, out_low with
+    low_bits 0, res_chan with res_kind 0, and the unused outputs of hawq_conv2d_dual, hawq_maxpool_requant and hawq_stem_pool_i8."""
+    r = rng(404)
+    n, h, w, cin, cout = 3, 7, 7, 64, 192                                  # M = 147: ragged last row tile, BN = 64
+    m = n * h * w
+    x = rand_act(r, m * cin, 8)
+    wt = torch.from_numpy(r.randint(-8, 8, size=(cout, 3, 3, cin)).astype(np.int8))
+    chan = make_chan(r, cout, ratio_lo=1e-2, ratio_hi=0.9)
+    d = ops.conv_desc(n, h, w, cin, cout, 3, 3, 1, 1, 8)
+    res32 = rand_act(r, m * cout, 32)
+    unused_res = dict(res=poisoned(m * cout, torch.int32), res_chan=poisoned(cout * 4, torch.int32).view(cout, 4))
+    unused_fs = dict(fscale=poisoned(cout, torch.float32))
+    unused_low = dict(out_low=poisoned(m * cout, torch.int8))
+    low8 = dict(low_bits=8, low_me=dyadic(0.004), low_clamp=(-128, 127))
+    cases = [   # epilogue, buffers, the outputs among them
+        (ops.epilogue(EPI_REQUANT, relu=1, out_bits=8, clamp=(-128, 127), flags=TC_FLAG),
+         dict(out=out_buf(m * cout, 8), **unused_res, **unused_fs, **unused_low), ["out"]),
+        (ops.epilogue(EPI_REQUANT, out_bits=32, clamp=(-2 ** 31, 2 ** 31 - 1)),
+         dict(out=out_buf(m * cout, 32), **unused_res, **unused_fs, **unused_low), ["out"]),
+        (ops.epilogue(EPI_RAW_I32), dict(out=out_buf(m * cout, 32), **unused_res, **unused_fs, **unused_low), ["out"]),
+        (ops.epilogue(EPI_DEQUANT_F32, cout_store=cout - 5),
+         dict(out=torch.zeros(m * (cout - 5)), fscale=torch.from_numpy(r.uniform(1e-5, 1e-3, size=cout).astype(np.float32)), **unused_res,
+              **unused_low), ["out"]),
+        (ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=0, res_bits=32, res_me=dyadic(0.37), y_bits=0, **low8, flags=TC_FLAG),
+         dict(res=res32, res_chan=unused_res["res_chan"], out=poisoned(m * cout, torch.int32), out_low=out_buf(m * cout, 8), **unused_fs), ["out_low"]),
+        (ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=0, res_bits=32, res_me=dyadic(0.37), y_bits=32),
+         dict(res=res32, res_chan=unused_res["res_chan"], out=out_buf(m * cout, 32), **unused_fs, **unused_low), ["out"]),
+        (ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=1, res_bits=32, y_bits=16, flags=TC_FLAG),
+         dict(res=res32, res_chan=make_chan(r, cout, ratio_lo=1e-2, ratio_hi=0.9), out=out_buf(m * cout, 16), **unused_fs, **unused_low), ["out"]),
+    ]
+    for ep, bufs, keys in cases:
+        run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, **bufs), keys)
+
+    # resize-unit kernel without a low-bit copy
+    x2 = rand_act(r, m * cin, 8)
+    w1 = torch.from_numpy(r.randint(-8, 8, size=(cout, 1, 1, cin)).astype(np.int8))
+    w2 = torch.from_numpy(r.randint(-8, 8, size=(cout, 1, 1, cin)).astype(np.int8))
+    d1 = ops.conv_desc(n, h, w, cin, cout, 1, 1, 1, 0, 8, 1)
+    ep = ops.epilogue(EPI_RESIDUAL, relu=1, res_kind=1, res_bits=32, y_bits=16, flags=TC_FLAG)
+    run_both("conv2d_dual", dict(x=x, desc=d1, ep=ep, w=w1, chan=chan, desc2=d1, x2=x2, w2=w2, chan2=make_chan(r, cout, ratio_lo=1e-2, ratio_hi=0.9),
+                                 out=out_buf(m * cout, 16), **unused_low), ["out"],
+             gpu_overrides=dict(w=ops.upload_weights(w1, DEV), w2=ops.upload_weights(w2, DEV)))
+
+    # max-pool + requant without the stream, and without the low-bit copy
+    ph, pw, c = 9, 11, 64
+    xp = torch.from_numpy(r.randint(0, 32768, size=2 * ph * pw * c).astype(np.int16))
+    pm = 2 * ((ph - 1) // 2 + 1) * ((pw - 1) // 2 + 1) * c
+    for y_bits, low_bits in [(0, 8), (16, 0), (32, 0)]:
+        args = dict(x=xp, n=2, hh=ph, ww=pw, c=c, y_bits=y_bits, y=out_buf(pm, y_bits or 32), low_bits=low_bits, low_me=dyadic(0.003),
+                    low_clamp=(-128, 127), out_low=out_buf(pm, 8))
+        if not y_bits:
+            args["y"] = poisoned(pm, torch.int32)
+        if not low_bits:
+            args["out_low"] = poisoned(pm, torch.int8)
+        run_both("maxpool_requant", args, ["y" if y_bits else "out_low"])
+
+    # fused stem without the low-bit copy (the stream is always written)
+    sh, sw = 17, 32
+    xs = torch.from_numpy(r.randint(-128, 128, size=2 * sh * sw * 3).astype(np.int8))
+    ws = torch.zeros((64, 8, 8, 4), dtype=torch.int8)
+    ws[:, :7, :7, :3] = torch.from_numpy(r.randint(-128, 128, size=(64, 7, 7, 3)).astype(np.int8))
+    po, qo = ((sh - 1) // 2) // 2 + 1, ((sw - 1) // 2) // 2 + 1
+    run_both("stem_pool", dict(x=xs, w256=ws, chan=make_chan(r, 64, ratio_lo=0.05, ratio_hi=0.8), clamp=(-32768, 32767), n=2, hh=sh, ww=sw, y_bits=16,
+                               y=out_buf(2 * po * qo * 64, 16), low_bits=0, low_me=(0, 1), low_clamp=(0, 0), out_low=poisoned(2 * po * qo * 64, torch.int8)),
+             ["y"])
 
 
 @pytest.mark.parametrize("shape", [(130, 2048, 1000, 1024), (128, 512, 10, 64), (3, 192, 100, 128), (1, 64, 64, 64)])
@@ -706,7 +813,8 @@ BOUNDARY_GEOMS = [
     (3, 9, 9, 128, 512, 1, 1, 1, 0),      # 1x1, M = 243: two row tiles
 ]
 REQUANT_CASES = [(out_bits, clamp, relu) for out_bits, clamp in [(4, (0, 15)), (8, (-128, 127)), (16, (-32768, 32767)), (32, (I32_MIN, I32_MAX))]
-                 for relu in (0, 1)] + [(8, (-128, -5), 1)]   # ReLU with clamp_hi < 0: every output is clamp_hi
+                 for relu in (0, 1)] + [(8, (-128, -5), 1),   # ReLU with clamp_hi < 0: every output is clamp_hi
+                                        (8, (-128, 0), 1)]    # ReLU with clamp_hi = 0: every output byte is 0
 RESIDUAL_CASES = [  # res_kind, res_bits, y_bits, low_bits, relu
     (0, 16, 16, 8, 1), (0, 32, 32, 4, 1), (0, 32, 32, 0, 0), (0, 16, 0, 4, 1), (1, 32, 16, 4, 1), (1, 32, 0, 8, 1), (1, 32, 32, 0, 0)]
 
@@ -730,8 +838,8 @@ def test_conv_epilogue_boundaries(geom, a_bits, flags):
         keys = [k_ for k_ in ("out", "out_low") if bufs.get(k_) is not None]
         try:
             cs, gs = run_both("conv2d", dict(x=x, desc=d, ep=ep, w=wt, chan=chan, **bufs), keys)
-        except AssertionError as status_mismatch:
-            failed.append((what, "status", str(status_mismatch)))
+        except AssertionError as mismatch:   # status word, output bytes, guards or inputs
+            failed.append((what, str(mismatch)))
             return
         for a, b, k_ in zip(cs, gs, keys):
             if not torch.equal(a, b):
