@@ -8,6 +8,7 @@
 #include <cstdlib>
 
 #include "conv_igemm.cuh"
+#include "conv_tail.cuh"
 #include "elementwise.cuh"
 #include "stem.cuh"
 
@@ -51,20 +52,21 @@ static int grid_for(long long work_items, int sm_count) {
 }
 
 // The maximum carveout lets the driver pick the 228 KB shared-memory configuration, the only one in which two CTAs of every
-// conv_igemm instantiation fit (ConvSmem's static_assert).
-template <int BN, bool A4, int FAM, bool DUAL>
-static int set_conv_attr1() {
-  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, FAM, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                ConvSmem<BN, A4, DUAL>::TOTAL));
-  CUDA_TRY(cudaFuncSetAttribute(conv_igemm_kernel<BN, A4, FAM, DUAL>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                cudaSharedmemCarveoutMaxShared));
+// conv_igemm and conv_tail instantiation fit (ConvSmem's and TailSmem's static_assert).
+template <class K>
+static int set_smem_attr(K* kernel, int smem) {
+  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   return HAWQ_OK;
 }
 template <int BN, bool A4>
 static int set_conv_attr() {
+  constexpr int smem = ConvSmem<BN, A4>::TOTAL;
   int rc;
-  if ((rc = set_conv_attr1<BN, A4, FAM_REQUANT, false>()) || (rc = set_conv_attr1<BN, A4, FAM_RESIDUAL, false>()) ||
-      (rc = set_conv_attr1<BN, A4, FAM_STORE, false>()))
+  if ((rc = set_smem_attr(conv_igemm_kernel<BN, A4, FAM_REQUANT>, smem)) || (rc = set_smem_attr(conv_igemm_kernel<BN, A4, FAM_RESIDUAL>, smem)) ||
+      (rc = set_smem_attr(conv_igemm_kernel<BN, A4, FAM_STORE>, smem)) ||
+      (rc = set_smem_attr(conv_tail_kernel<A4, false>, TailSmem<A4, false>::TOTAL)) ||
+      (rc = set_smem_attr(conv_tail_kernel<A4, true>, TailSmem<A4, true>::TOTAL)))
     return rc;
   return HAWQ_OK;
 }
@@ -74,16 +76,16 @@ static dim3 conv_grid(long long M, int Cout, int BN) { return dim3((unsigned)((M
 
 template <int BN, bool A4>
 static void launch_conv(const ConvParams& p, cudaStream_t s) {
-  const int smem = ConvSmem<BN, A4, false>::TOTAL;
+  const int smem = ConvSmem<BN, A4>::TOTAL;
   const dim3 grid = conv_grid(p.M, p.Cout, BN);
-  if (p.mode == HAWQ_EPI_REQUANT) conv_igemm_kernel<BN, A4, FAM_REQUANT, false><<<grid, CONV_THREADS, smem, s>>>(p);
-  else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, FAM_RESIDUAL, false><<<grid, CONV_THREADS, smem, s>>>(p);
-  else conv_igemm_kernel<BN, A4, FAM_STORE, false><<<grid, CONV_THREADS, smem, s>>>(p);
+  if (p.mode == HAWQ_EPI_REQUANT) conv_igemm_kernel<BN, A4, FAM_REQUANT><<<grid, CONV_THREADS, smem, s>>>(p);
+  else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, FAM_RESIDUAL><<<grid, CONV_THREADS, smem, s>>>(p);
+  else conv_igemm_kernel<BN, A4, FAM_STORE><<<grid, CONV_THREADS, smem, s>>>(p);
 }
-// resize units always run at BN = 64: the int32 identity tile of BN = 128 would leave room for one CTA per SM
-template <bool A4>
-static void launch_conv_dual(const ConvParams& p, cudaStream_t s) {
-  conv_igemm_kernel<64, A4, FAM_RESIDUAL, true><<<conv_grid(p.M, p.Cout, 64), CONV_THREADS, ConvSmem<64, A4, true>::TOTAL, s>>>(p);
+// persistent tail kernel: bottleneck tails (DUAL = false) and resize units (DUAL = true)
+template <bool A4, bool DUAL>
+static void launch_conv_tail(const ConvParams& p, int sm_count, cudaStream_t s) {
+  conv_tail_kernel<A4, DUAL><<<tail_grid(p.Cout, sm_count), CONV_THREADS, TailSmem<A4, DUAL>::TOTAL, s>>>(p);
 }
 
 extern "C" {
@@ -107,8 +109,7 @@ int hawq_create(int device, hawq_handle** out) {
   int rc;
   CUDA_TRY(cudaFuncSetAttribute(linear_dp4a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, linear_smem_bytes(LIN_MAX_K)));
   if ((rc = set_conv_attr<128, false>()) || (rc = set_conv_attr<64, false>()) || (rc = set_conv_attr<128, true>()) ||
-      (rc = set_conv_attr<64, true>()) || (rc = set_conv_attr1<64, false, FAM_RESIDUAL, true>()) ||
-      (rc = set_conv_attr1<64, true, FAM_RESIDUAL, true>()))
+      (rc = set_conv_attr<64, true>()))
     return rc;
   *out = h;
   return HAWQ_OK;
@@ -165,6 +166,7 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
   if (d->a_bits != 8 && d->a_bits != 4) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: a_bits must be 4 or 8");
   if (d->Cin % 64 != 0 || d->Cout % 64 != 0)
     return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: Cin (%d) and Cout (%d) must be multiples of 64", d->Cin, d->Cout);
+  if (d->Cin < 64 || d->Cout < 64) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: Cin (%d) and Cout (%d) must be at least 64", d->Cin, d->Cout);
   const int Ho = (d->H + 2 * d->pad - d->kh) / d->stride + 1;
   const int Wo = (d->W + 2 * d->pad - d->kw) / d->stride + 1;
   if (Ho < 1 || Wo < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: empty output");
@@ -234,7 +236,13 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
     return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: more than 2^31 - 1 output tiles");
   ++g_kernel_count[0];
   cudaStream_t s = (cudaStream_t)stream;
-  if (d->a_bits == 8) {
+  // bottleneck tails (1x1 stride 1, uint16 residual operand and stream): the persistent tail kernel
+  const bool tail = ep->mode == HAWQ_EPI_RESIDUAL && d->kh == 1 && d->kw == 1 && d->stride == 1 && d->pad == 0 && ep->res_kind == 0 &&
+                    ep->res_bits == 16 && ep->y_bits == 16;
+  if (tail) {
+    if (d->a_bits == 8) launch_conv_tail<false, false>(p, h->sm_count, s);
+    else launch_conv_tail<true, false>(p, h->sm_count, s);
+  } else if (d->a_bits == 8) {
     if (bn128) launch_conv<128, false>(p, s);
     else launch_conv<64, false>(p, s);
   } else {
@@ -245,7 +253,8 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
 }
 
 // Resize-unit fusion: y = RHE(m1 * (conv1x1_s(x2, w2) + bias2)) + RHE(m * (conv1x1(x, w) + bias)), ReLU, uint16 stream +
-// optional low-bit copy.  Both convolutions run in one kernel; the identity result stays in shared memory (no int32 tensor in HBM).
+// optional low-bit copy.  Both convolutions run in one kernel (conv_tail.cuh); each thread parks its requantised identity terms in
+// shared memory until the main convolution's epilogue (no int32 tensor in HBM).
 int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_desc* ep, const void* x, const int8_t* w,
                      const hawq_chan* chan, const hawq_conv_desc* d2, const void* x2, const int8_t* w2, const hawq_chan* chan2,
                      void* out, void* out_low, void* stream) {
@@ -255,6 +264,7 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
   if (d->N < 1 || d->H < 1 || d->W < 1 || d2->H < 1 || d2->W < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: bad geometry");
   if ((d->a_bits != 8 && d->a_bits != 4) || d2->a_bits != d->a_bits) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: a_bits must be equal and 4 or 8");
   if (d->Cin % 64 || d2->Cin % 64 || d->Cout % 64 || d2->Cout != d->Cout) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: channel counts must be multiples of 64 and Cout equal");
+  if (d->Cin < 64 || d2->Cin < 64 || d->Cout < 64) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: Cin and Cout must be at least 64");
   if (d2->N != d->N || (d2->H - 1) / d2->stride + 1 != d->H || (d2->W - 1) / d2->stride + 1 != d->W)
     return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: the two convolutions have different output grids");
   if (d->w_layout != 1 || d2->w_layout != 1) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: weights must carry the re-tiled copy (w_layout 1)");
@@ -288,8 +298,8 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
   p.x2_pix_bytes = d2->Cin * d2->a_bits / 8;
 
   cudaStream_t s = (cudaStream_t)stream;
-  if (d->a_bits == 8) launch_conv_dual<false>(p, s);
-  else launch_conv_dual<true>(p, s);
+  if (d->a_bits == 8) launch_conv_tail<false, true>(p, h->sm_count, s);
+  else launch_conv_tail<true, true>(p, h->sm_count, s);
   return launch_check("conv_dual");
 }
 

@@ -10,9 +10,6 @@
 //   two int8x4 words of the register A fragment.  The weight rows of such layers are K-permuted on the host so that the
 //   expansion needs no shuffles (hawq_permute_weights_for_i4).
 //
-//   DUAL = true (resize units): the identity-branch 1x1 convolution (x2, w2) runs first in the same CTA; its int32 result
-//   (acc + bias2) stays in shared memory as the res_kind 1 operand of the RESIDUAL epilogue of the main convolution.
-//
 //   Epilogues (hawq_epilogue_mode), one instantiation per family: REQUANT (case 0 of fixedpoint_fn), RESIDUAL (case 1: dual
 //   dyadic requant + add, optional ReLU, writes the new residual stream and/or the next unit's low-bit activation), and STORE
 //   (RAW_I32, DEQUANT_F32).  The REQUANT and RESIDUAL bodies are written once, over a requantisation implementation that each
@@ -50,7 +47,7 @@ struct ConvParams {
   int scalar_unchecked;  // host-checked: the scalar residual ratio exceeds 2^20 or the low-bit ratio exceeds 1 (no checked FP64 form)
   int check_ovf;     // RESIDUAL under a HAWQ_EP_RATIOS_* promise: a requantised term leaving int32 raises HAWQ_FLAG_REQUANT_OVERFLOW
   int bias_lo, bias_hi;   // host-computed from K and a_bits: a bias in [bias_lo, bias_hi] keeps acc + bias inside int32 (empty when bias_lo > bias_hi)
-  // DUAL launches: the identity 1x1 convolution (res_chan holds its bias and per-channel identity ratio)
+  // resize units (conv_tail.cuh): the identity 1x1 convolution (res_chan holds its bias and per-channel identity ratio)
   const uint8_t* x2;
   const int8_t* w2;
   int H2, W2, stride2, cin_chunks2, x2_pix_bytes;
@@ -60,16 +57,32 @@ constexpr int CONV_BM = 128;
 constexpr int CONV_STAGES = 4;
 constexpr int CONV_THREADS = 256;
 
+// Per-channel arrays of a CTA's channel block (BN channels), behind the tiles of its shared memory.
+template <int BN>
+struct ChanSmem {
+  static constexpr int M_OFF = BN * (int)sizeof(hawq_chan);    // double[BN]: m * 2^-e of chan
+  static constexpr int M1_OFF = M_OFF + BN * 8;                // double[BN]: m * 2^-e of res_chan
+  static constexpr int RC_OFF = M1_OFF + BN * 8;               // hawq_chan[BN]: res_chan
+  static constexpr int CB_OFF = RC_OFF + BN * (int)sizeof(hawq_chan);   // double[BN]: 2^52 + 2^31 - bias
+  static constexpr int BYTES = CB_OFF + BN * 8;
+  hawq_chan* chan;
+  double* M;
+  double* M1;
+  hawq_chan* rc;
+  double* Cb;
+  __device__ explicit ChanSmem(uint8_t* base)
+      : chan(reinterpret_cast<hawq_chan*>(base)), M(reinterpret_cast<double*>(base + M_OFF)),
+        M1(reinterpret_cast<double*>(base + M1_OFF)), rc(reinterpret_cast<hawq_chan*>(base + RC_OFF)),
+        Cb(reinterpret_cast<double*>(base + CB_OFF)) {}
+};
+
 // Shared memory of one CTA.  The cp.async ring is free once the GEMM has drained, so the epilogue tiles reuse it:
-//   non-DUAL  [ ring | uint16 residual tile ] [ channel arrays ]
-//             The uint16 residual tile has its own region: it is prefetched while the ring is in use (see gemm()).
-//             After the GEMM the low-bit staging tile takes ring offset 0, and an int32 residual operand (loaded only after
-//             the GEMM) starts right behind it, across the rest of the ring and the uint16 region.
-//   DUAL      [ ring | int32 identity tile ] [ channel arrays ]
-//             The identity tile is written after the identity GEMM and read by the main convolution's epilogue.  After the
-//             main GEMM the low-bit tile (offset 0) and the uint16 stream tile (Y_OFF) are staged in the ring.
+//   [ ring | uint16 residual tile ] [ channel arrays ]
+//   The uint16 residual tile has its own region: it is prefetched while the ring is in use (see gemm()).  After the GEMM the
+//   low-bit staging tile takes ring offset 0, and an int32 residual operand (loaded only after the GEMM) starts right behind it,
+//   across the rest of the ring and the uint16 region.
 // Two CTAs per SM (what __launch_bounds__(CONV_THREADS, 2) plans for) need 2 * (TOTAL + 1 KB reserved per CTA) <= 228 KB.
-template <int BN, bool A4, bool DUAL>
+template <int BN, bool A4>
 struct ConvSmem {
   static constexpr int A_ROW = A4 ? 32 : 64;  // bytes of one A row per k-tile (64 channels)
   static constexpr int A_STAGE = CONV_BM * A_ROW;
@@ -77,19 +90,14 @@ struct ConvSmem {
   static constexpr int PIPE = CONV_STAGES * (A_STAGE + B_STAGE);
   static constexpr int OUT_PITCH = BN + 16;
   static constexpr int OUT_STAGE = CONV_BM * OUT_PITCH;                    // low-bit output staging tile, at offset 0
-  static constexpr int RES16 = CONV_BM * (BN * 2 + 16);                    // uint16 tile (residual operand or stream), padded pitch
+  static constexpr int RES16 = CONV_BM * (BN * 2 + 16);                    // uint16 residual tile, padded pitch
   static constexpr int RES32 = CONV_BM * (BN * 4 + 32);                    // int32 tile, padded pitch
   static constexpr int RES16_OFF = PIPE;
-  static constexpr int RES32_OFF = DUAL ? PIPE : OUT_STAGE;
-  static constexpr int Y_OFF = OUT_STAGE;                                  // DUAL: staged uint16 stream tile
-  static constexpr int MAIN = DUAL ? PIPE + RES32 : (PIPE + RES16 > RES32_OFF + RES32 ? PIPE + RES16 : RES32_OFF + RES32);
-  static constexpr int CHAN_OFF = MAIN;                                    // hawq_chan[BN]
-  static constexpr int M_OFF = CHAN_OFF + BN * (int)sizeof(hawq_chan);     // double[BN]: m * 2^-e of chan
-  static constexpr int M1_OFF = M_OFF + BN * 8;                           // double[BN]: m * 2^-e of res_chan
-  static constexpr int RC_OFF = M1_OFF + BN * 8;                          // hawq_chan[BN]: res_chan
-  static constexpr int CB_OFF = RC_OFF + BN * (int)sizeof(hawq_chan);     // double[BN]: 2^52 + 2^31 - bias
-  static constexpr int TOTAL = CB_OFF + BN * 8;
-  static_assert(OUT_STAGE <= PIPE && (!DUAL || Y_OFF + RES16 <= PIPE), "the epilogue staging tiles must fit in the freed ring");
+  static constexpr int RES32_OFF = OUT_STAGE;
+  static constexpr int MAIN = PIPE + RES16 > RES32_OFF + RES32 ? PIPE + RES16 : RES32_OFF + RES32;
+  static constexpr int CHAN_OFF = MAIN;
+  static constexpr int TOTAL = CHAN_OFF + ChanSmem<BN>::BYTES;
+  static_assert(OUT_STAGE <= PIPE, "the low-bit staging tile must fit in the freed ring");
   static_assert(2 * (TOTAL + 1024) <= 228 * 1024, "two CTAs per SM must fit in shared memory");
 };
 
@@ -100,7 +108,7 @@ __device__ __forceinline__ int swz(int row, int ch) {
   else return row * 32 + ((ch ^ ((row >> 2) & 1)) << 4);
 }
 
-// Epilogue family of an instantiation (FAM): REQUANT to 4/8/16/32 bits, RESIDUAL (DUAL launches included), STORE (RAW_I32 and
+// Epilogue family of an instantiation (FAM): REQUANT to 4/8/16/32 bits, RESIDUAL, STORE (RAW_I32 and
 // DEQUANT_F32, no requantisation).  A kernel carries its own family's body only.
 constexpr int FAM_REQUANT = 0, FAM_RESIDUAL = 1, FAM_STORE = 2;
 
@@ -150,16 +158,122 @@ struct RqExact {
   }
 };
 
-// geometry of one implicit GEMM of a launch (the main convolution, or the identity convolution of a DUAL launch)
+// Requantisation policy of a CTA, from its channel block and the launch's scalar ratios: FP64 when every ratio is <= 1, and for
+// RESIDUAL under a ratio promise when every ratio is <= 2^20 (the low-bit ratio <= 1), each term then checked; Exact otherwise.
+// An FP64 CTA with a bias outside the window clamps.
+struct RqPolicy {
+  bool over_one;    // some ratio > 1
+  bool unchecked;   // some ratio > 2^20 (or a low-bit ratio > 1): beyond the checked FP64 form
+  bool clamped;     // some bias outside [bias_lo, bias_hi]: acc + bias may leave int32
+};
+
+// Loads the channel block n0 ... n0 + BN - 1 (and, for a res_kind 1 RESIDUAL, its res_chan) into shared memory and returns the
+// CTA's policy.  Every thread of the CTA must call it (three __syncthreads_or).
+template <int BN, bool RESIDUAL>
+__device__ RqPolicy load_channel_block(const ConvParams& p, int n0, const ChanSmem<BN>& cs) {
+  int over_one = p.scalar_over_one, unchecked = p.scalar_unchecked, bias_out = 0;
+  const int tid = threadIdx.x;
+  if (tid < BN) {
+    const hawq_chan c = p.chan[n0 + tid];
+    cs.chan[tid] = c;
+    cs.M[tid] = dyadic_to_double(c.m, c.e);
+    cs.Cb[tid] = 4503601774854144.0 - (double)c.bias;   // exact: folds the bias add into the int -> double conversion
+    bias_out = c.bias < p.bias_lo || c.bias > p.bias_hi;
+    over_one |= !dyadic_is_fast(c.m, c.e);
+    unchecked |= !dyadic_is_wide(c.m, c.e);
+    if (RESIDUAL && p.res_kind == 1) {
+      const hawq_chan rc = p.res_chan[n0 + tid];
+      cs.rc[tid] = rc;
+      cs.M1[tid] = dyadic_to_double(rc.m, rc.e);
+      over_one |= !dyadic_is_fast(rc.m, rc.e);
+      unchecked |= !dyadic_is_wide(rc.m, rc.e);
+    }
+  }
+  RqPolicy pol;
+  pol.over_one = __syncthreads_or(over_one) != 0;
+  pol.unchecked = __syncthreads_or(unchecked) != 0;
+  pol.clamped = __syncthreads_or(bias_out) != 0;
+  return pol;
+}
+
+// Calls f with the requantisation implementation of the policy (RqExact, RqFp64<true> or RqFp64<false>), checked as RESIDUAL needs.
+template <bool RESIDUAL, class F>
+__device__ __forceinline__ void with_rq(const RqPolicy& pol, const ConvParams& p, F&& f) {
+  const bool fp64 = !pol.over_one || (RESIDUAL && p.check_ovf && !pol.unchecked);
+  if (!fp64) f(RqExact{RESIDUAL && p.check_ovf != 0});
+  else if (pol.clamped) f(RqFp64<true>{RESIDUAL && pol.over_one});
+  else f(RqFp64<false>{RESIDUAL && pol.over_one});
+}
+
+// RESIDUAL epilogue of one output: y = [ReLU](sat_add(res_term, RHE((acc + bias) * ratio))), where res_term = RHE(r * ratio1) of
+// the residual operand r; with `ok` (a real row) a term leaving int32 counts for HAWQ_FLAG_REQUANT_OVERFLOW.
+template <class Rq>
+__device__ __forceinline__ int32_t residual_y(Rq& rq, int32_t res_term, int32_t acc, double cb, const int4& c, double M, bool ok,
+                                              int32_t relu_floor) {
+  return max(sat_add(res_term, rq.term(rq.acc_bias(acc, cb, c.x), M, c.y, c.z, ok)), relu_floor);
+}
+// the low-bit copy of y for the next unit: clamp(RHE(y * low ratio))
+template <class Rq>
+__device__ __forceinline__ int32_t residual_low(Rq& rq, int32_t y, double low_M, const ConvParams& p) {
+  return clampi(rq.term(rq.of_i32(y), low_M, p.low_m, p.low_e, false), p.low_lo, p.low_hi);
+}
+// a pair of the uint16 stream: saturates at 65535; ymax keeps the largest value of real rows for HAWQ_FLAG_RESIDUAL_OVERFLOW
+__device__ __forceinline__ uint32_t stream16_pair(int32_t y0, int32_t y1, bool ok, int& ymax) {
+  if (ok) ymax = max(ymax, max(y0, y1));
+  return (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
+}
+__device__ __forceinline__ void residual_flags(const ConvParams& p, int ymax, bool ovf) {
+  if (ymax > 65535) atomicOr(p.status, HAWQ_FLAG_RESIDUAL_OVERFLOW);
+  if (ovf) atomicOr(p.status, HAWQ_FLAG_REQUANT_OVERFLOW);
+}
+// a pair of low-bit outputs (columns col, col + 1) into a staging tile of one byte per value
+__device__ __forceinline__ void stage_low_pair(uint8_t* s, int pitch, int row, int col, int q0, int q1) {
+  *reinterpret_cast<uint16_t*>(s + row * pitch + col) = (uint16_t)__byte_perm(q0, q1, 0x0040);
+}
+
+// Coalesced 16-byte copy-out of a staged tile of CONV_BM rows: row r (row_bytes at s + r * s_pitch) goes to g + (m0 + r) * g_pitch;
+// rows at or past M are skipped.  The caller synchronises before.
+__device__ __forceinline__ void copy_out_rows(const uint8_t* s, int s_pitch, uint8_t* g, size_t g_pitch, int row_bytes, int m0, int M) {
+  const int cpr = row_bytes / 16;
+  for (int id = threadIdx.x; id < CONV_BM * cpr; id += blockDim.x) {
+    const int row = id / cpr, j = id - row * cpr;
+    if (m0 + row < M)
+      *reinterpret_cast<int4*>(g + (size_t)(m0 + row) * g_pitch + j * 16) = *reinterpret_cast<const int4*>(s + row * s_pitch + j * 16);
+  }
+}
+// The low-bit staging tile (one byte per value, BN columns) -> 8-bit rows, or 4-bit rows packed in hawq nibble order.
+template <int BN>
+__device__ __forceinline__ void copy_out_low(const uint8_t* s, int pitch, uint8_t* gout, int bits, int m0, int n0, int M, int Cout) {
+  if (bits == 8) {
+    copy_out_rows(s, pitch, gout + n0, (size_t)Cout, BN, m0, M);
+  } else {  // 32 channels -> 16 packed bytes
+    constexpr int CPR = BN / 32;
+    for (int id = threadIdx.x; id < CONV_BM * CPR; id += blockDim.x) {
+      const int row = id / CPR, j = id % CPR;
+      if (m0 + row < M) {
+        const uint4 a = *reinterpret_cast<const uint4*>(s + row * pitch + j * 32);
+        const uint4 b = *reinterpret_cast<const uint4*>(s + row * pitch + j * 32 + 16);
+        uint4 o;
+        o.x = pack_nibbles8(a.x, a.y);
+        o.y = pack_nibbles8(a.z, a.w);
+        o.z = pack_nibbles8(b.x, b.y);
+        o.w = pack_nibbles8(b.z, b.w);
+        *reinterpret_cast<uint4*>(gout + (((size_t)(m0 + row) * Cout + n0 + j * 32) >> 1)) = o;
+      }
+    }
+  }
+}
+
+// geometry of the implicit GEMM of a launch
 struct ConvGeom {
   const uint8_t* x;
   const int8_t* w;
   int H, W, stride, pad, KH, KW, cin_chunks, x_pix_bytes, K;
 };
 
-template <int BN, bool A4, int FAM, bool DUAL>
+template <int BN, bool A4, int FAM>
 __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvParams p) {
-  using S = ConvSmem<BN, A4, DUAL>;
+  using S = ConvSmem<BN, A4>;
   constexpr int BM = CONV_BM, STAGES = CONV_STAGES;
   constexpr int A_ROW = S::A_ROW;
   constexpr int A_CH = A_ROW / 16;                    // 16-byte chunks per A row: 4 or 2
@@ -172,11 +286,12 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   extern __shared__ __align__(1024) uint8_t smem[];   // 512-B aligned tiles: the wgmma descriptors address them swizzled
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * S::A_STAGE;
-  hawq_chan* sChan = reinterpret_cast<hawq_chan*>(smem + S::CHAN_OFF);
-  double* sM = reinterpret_cast<double*>(smem + S::M_OFF);
-  double* sM1 = reinterpret_cast<double*>(smem + S::M1_OFF);
-  hawq_chan* sResChan = reinterpret_cast<hawq_chan*>(smem + S::RC_OFF);
-  double* sCb = reinterpret_cast<double*>(smem + S::CB_OFF);
+  const ChanSmem<BN> cs(smem + S::CHAN_OFF);
+  const hawq_chan* sChan = cs.chan;
+  const double* sM = cs.M;
+  const double* sM1 = cs.M1;
+  const hawq_chan* sResChan = cs.rc;
+  const double* sCb = cs.Cb;
 
   const int tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5;
@@ -188,31 +303,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   const int m0 = (int)(blockIdx.x / nblk) * BM;
   const int n0 = (int)(blockIdx.x % nblk) * BN;
 
-  int over_one = p.scalar_over_one;     // some ratio > 1
-  int unchecked = p.scalar_unchecked;   // some ratio > 2^20 (or a low-bit ratio > 1): beyond the checked FP64 form
-  int bias_out = 0;                     // some bias outside [bias_lo, bias_hi]: acc + bias may leave int32
-  if (tid < BN) {
-    const hawq_chan c = p.chan[n0 + tid];
-    sChan[tid] = c;
-    sM[tid] = dyadic_to_double(c.m, c.e);
-    sCb[tid] = 4503601774854144.0 - (double)c.bias;   // exact: folds the bias add into the int -> double conversion
-    bias_out = c.bias < p.bias_lo || c.bias > p.bias_hi;
-    over_one |= !dyadic_is_fast(c.m, c.e);
-    unchecked |= !dyadic_is_wide(c.m, c.e);
-    if (FAM == FAM_RESIDUAL && p.res_kind == 1) {
-      const hawq_chan rc = p.res_chan[n0 + tid];
-      sResChan[tid] = rc;
-      sM1[tid] = dyadic_to_double(rc.m, rc.e);
-      over_one |= !dyadic_is_fast(rc.m, rc.e);
-      unchecked |= !dyadic_is_wide(rc.m, rc.e);
-    }
-  }
-  // Requantisation policy, CTA-uniform: FP64 when every ratio is <= 1, and for RESIDUAL under a ratio promise when every ratio is
-  // <= 2^20 (the low-bit ratio <= 1), each term then checked; Exact otherwise.  An FP64 CTA with a bias outside the window clamps.
-  const bool ratio_over_one = __syncthreads_or(over_one) != 0;
-  const bool ratio_unchecked = __syncthreads_or(unchecked) != 0;
-  const bool clamped = __syncthreads_or(bias_out) != 0;
-  const bool fp64 = !ratio_over_one || (FAM == FAM_RESIDUAL && p.check_ovf && !ratio_unchecked);
+  const RqPolicy pol = load_channel_block<BN, FAM == FAM_RESIDUAL>(p, n0, cs);
 
   int32_t acc[NACC];
 
@@ -235,7 +326,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
     }
   };
   // the uint16 residual operand has its own region: it is fetched while the GEMM runs (the int32 operand overlaps the ring)
-  const bool prefetch_res = !DUAL && res_es == 2;
+  const bool prefetch_res = res_es == 2;
 
   // acc = A(128 x K) * B(K x BN) of geometry gm for this CTA's tile; with_res: the residual tile joins the prologue
   auto gemm = [&](const ConvGeom& gm, bool with_res) {
@@ -332,52 +423,34 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
     __syncthreads();   // pipeline buffers are free
   };
 
-  if constexpr (DUAL) {   // identity convolution first: acc + bias2 (saturating) is the int32 res_kind 1 operand
-    gemm(ConvGeom{p.x2, p.w2, p.H2, p.W2, p.stride2, 0, 1, 1, p.cin_chunks2, p.x2_pix_bytes, p.cin_chunks2 * 64}, false);
-#pragma unroll
-    for (int ni = 0; ni < NT; ++ni) {
-      const int col = ni * 8 + 2 * t;
-      const int b0 = sResChan[col].bias, b1 = sResChan[col + 1].bias;
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        const int row = warp * 16 + hf * 8 + g;
-        *reinterpret_cast<int2*>(sRes + row * res_pitch + col * 4) =
-            make_int2(sat_add(acc[ni * 4 + hf * 2], b0), sat_add(acc[ni * 4 + hf * 2 + 1], b1));
-      }
-    }
-  }
   gemm(ConvGeom{p.x, p.w, p.H, p.W, p.stride, p.pad, p.KH, p.KW, p.cin_chunks, p.x_pix_bytes, p.K}, prefetch_res);
 
-  if (!DUAL && res_es == 4) {   // int32 residual operand: its tile overlaps the ring, so it is loaded now
+  if (res_es == 4) {   // int32 residual operand: its tile overlaps the ring, so it is loaded now
     load_res();
     cp_async_commit();
     cp_async_wait<0>();
     __syncthreads();
   }
-  // the new residual stream is staged in shared memory and written with 16-byte stores: in place over the operand tile
-  // when both have the same width, in the freed ring in DUAL launches (uint16 stream over an int32 identity tile)
-  const bool y_staged = DUAL || (res_es != 0 && p.y_bits == res_es * 8);
+  // the new residual stream is staged in shared memory and written with 16-byte stores, in place over the operand tile when both
+  // have the same width
+  const bool y_staged = res_es != 0 && p.y_bits == res_es * 8;
   const int y_es = p.y_bits / 8;
   const int y_pitch = BN * y_es + 8 * y_es;
-  uint8_t* sY = DUAL ? smem + S::Y_OFF : sRes;
+  uint8_t* sY = sRes;
 
   // ------------------------------------------------------------------------------------------------ epilogue
   uint8_t* sOut = smem;
   const bool stage_low = (FAM == FAM_REQUANT && p.out_bits <= 8) || (FAM == FAM_RESIDUAL && p.low_bits != 0);
   const int stage_bits = (FAM == FAM_REQUANT) ? p.out_bits : p.low_bits;
 
-  // a pair of low-bit outputs (columns col, col + 1) into the staging tile
-  auto put_low = [&](int row, int col, int q0, int q1) {
-    *reinterpret_cast<uint16_t*>(sOut + row * S::OUT_PITCH + col) = (uint16_t)__byte_perm(q0, q1, 0x0040);
-  };
-  // a pair of the new residual stream, staged or stored directly; a uint16 stream saturates at 65535, and ymax keeps the largest
-  // value of the thread's real rows for HAWQ_FLAG_RESIDUAL_OVERFLOW
+  auto put_low = [&](int row, int col, int q0, int q1) { stage_low_pair(sOut, S::OUT_PITCH, row, col, q0, q1); };
+  // a pair of the new residual stream, staged or stored directly
   auto put_y = [&](int row, int col, bool ok, int y0, int y1, int& ymax) {
-    if (p.y_bits == 16 && ok) ymax = max(ymax, max(y0, y1));
+    const uint32_t y16 = p.y_bits == 16 ? stream16_pair(y0, y1, ok, ymax) : 0u;
     if (!y_staged && !ok) return;
     uint8_t* dst = y_staged ? sY + row * y_pitch + col * y_es
                             : reinterpret_cast<uint8_t*>(p.out) + ((size_t)(m0 + row) * p.Cout + n0 + col) * y_es;
-    if (p.y_bits == 16) *reinterpret_cast<uint32_t*>(dst) = (uint32_t)min(y0, 65535) | ((uint32_t)min(y1, 65535) << 16);
+    if (p.y_bits == 16) *reinterpret_cast<uint32_t*>(dst) = y16;
     else if (p.y_bits == 32) *reinterpret_cast<int2*>(dst) = make_int2(y0, y1);
   };
 
@@ -444,18 +517,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
             r0 = rq.of_i32(pr.x);
             r1 = rq.of_i32(pr.y);
           }
-          const auto v0 = rq.acc_bias(acc[ni * 4 + hf * 2 + 0], Cb.x, c0.x);
-          const auto v1 = rq.acc_bias(acc[ni * 4 + hf * 2 + 1], Cb.y, c1.x);
-          const int y0 = max(sat_add(rq.term(r0, M1.x, m1.x, e1.x, ok), rq.term(v0, M.x, c0.y, c0.z, ok)), relu_floor);
-          const int y1 = max(sat_add(rq.term(r1, M1.y, m1.y, e1.y, ok), rq.term(v1, M.y, c1.y, c1.z, ok)), relu_floor);
+          const int y0 = residual_y(rq, rq.term(r0, M1.x, m1.x, e1.x, ok), acc[ni * 4 + hf * 2 + 0], Cb.x, c0, M.x, ok, relu_floor);
+          const int y1 = residual_y(rq, rq.term(r1, M1.y, m1.y, e1.y, ok), acc[ni * 4 + hf * 2 + 1], Cb.y, c1, M.y, ok, relu_floor);
           put_y(row, col, ok, y0, y1, ymax);
-          if (p.low_bits != 0)
-            put_low(row, col, clampi(rq.term(rq.of_i32(y0), low_M, p.low_m, p.low_e, false), p.low_lo, p.low_hi),
-                    clampi(rq.term(rq.of_i32(y1), low_M, p.low_m, p.low_e, false), p.low_lo, p.low_hi));
+          if (p.low_bits != 0) put_low(row, col, residual_low(rq, y0, low_M, p), residual_low(rq, y1, low_M, p));
         }
       }
-      if (ymax > 65535) atomicOr(p.status, HAWQ_FLAG_RESIDUAL_OVERFLOW);
-      if (rq.ovf) atomicOr(p.status, HAWQ_FLAG_REQUANT_OVERFLOW);
+      residual_flags(p, ymax, rq.ovf);
     }
   };
 
@@ -480,54 +548,16 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       }
     }
   } else {
-    auto run = [&](auto low_out) {
-      if (!fp64) epilogue(RqExact{FAM == FAM_RESIDUAL && p.check_ovf}, low_out);
-      else if (clamped) epilogue(RqFp64<true>{FAM == FAM_RESIDUAL && ratio_over_one}, low_out);
-      else epilogue(RqFp64<false>{FAM == FAM_RESIDUAL && ratio_over_one}, low_out);
-    };
+    auto run = [&](auto low_out) { with_rq<FAM == FAM_RESIDUAL>(pol, p, [&](auto rq) { epilogue(rq, low_out); }); };
     if (FAM == FAM_REQUANT && p.out_bits <= 8) run(std::true_type{});
     else run(std::false_type{});
   }
 
   if (y_staged || stage_low) __syncthreads();
-  if (y_staged) {   // coalesced copy-out of the new residual stream tile
-    const int cpr = BN * y_es / 16;
-    uint8_t* gy = reinterpret_cast<uint8_t*>(p.out);
-    for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
-      const int row = id / cpr, j = id - row * cpr;
-      if (m0 + row < p.M)
-        *reinterpret_cast<int4*>(gy + ((size_t)(m0 + row) * p.Cout + n0) * y_es + j * 16) =
-            *reinterpret_cast<const int4*>(sY + row * y_pitch + j * 16);
-    }
-  }
-  if (stage_low) {
-    uint8_t* gout = reinterpret_cast<uint8_t*>(FAM == FAM_REQUANT ? p.out : p.out_low);
-    if (stage_bits == 8) {
-      constexpr int CPR = BN / 16;
-      for (int id = tid; id < BM * CPR; id += CONV_THREADS) {
-        const int row = id / CPR, j = id % CPR;
-        if (m0 + row < p.M) {
-          const int4 v = *reinterpret_cast<const int4*>(sOut + row * S::OUT_PITCH + j * 16);
-          *reinterpret_cast<int4*>(gout + (size_t)(m0 + row) * p.Cout + n0 + j * 16) = v;
-        }
-      }
-    } else {  // 4-bit: 32 channels -> 16 packed bytes
-      constexpr int CPR = BN / 32;
-      for (int id = tid; id < BM * CPR; id += CONV_THREADS) {
-        const int row = id / CPR, j = id % CPR;
-        if (m0 + row < p.M) {
-          const uint4 a = *reinterpret_cast<const uint4*>(sOut + row * S::OUT_PITCH + j * 32);
-          const uint4 b = *reinterpret_cast<const uint4*>(sOut + row * S::OUT_PITCH + j * 32 + 16);
-          uint4 o;
-          o.x = pack_nibbles8(a.x, a.y);
-          o.y = pack_nibbles8(a.z, a.w);
-          o.z = pack_nibbles8(b.x, b.y);
-          o.w = pack_nibbles8(b.z, b.w);
-          *reinterpret_cast<uint4*>(gout + (((size_t)(m0 + row) * p.Cout + n0 + j * 32) >> 1)) = o;
-        }
-      }
-    }
-  }
+  if (y_staged)   // coalesced copy-out of the new residual stream tile
+    copy_out_rows(sY, y_pitch, reinterpret_cast<uint8_t*>(p.out) + (size_t)n0 * y_es, (size_t)p.Cout * y_es, BN * y_es, m0, p.M);
+  if (stage_low)
+    copy_out_low<BN>(sOut, S::OUT_PITCH, reinterpret_cast<uint8_t*>(FAM == FAM_REQUANT ? p.out : p.out_low), stage_bits, m0, n0, p.M, p.Cout);
 }
 
 }  // namespace hawq
