@@ -1,10 +1,10 @@
-"""hawq_b200 — H100-native integer inference engine for HAWQ-quantized ResNets.
+"""hawq_b200 — H100-native integer inference engine for HAWQ-quantized ResNets and MobileNetV2.
 
 Public surface (mirrors the reference's module API for the quantized forward path):
   modules      QuantAct, QuantBnConv2d, QuantConv2d, QuantLinear, QuantAveragePool2d, QuantMaxPool2d, QuantDropout,
                freeze_model, unfreeze_model
   q_resnet     q_resnet18 / q_resnet50 / q_resnet101 (same module names / state_dict keys as the reference)
-  q_mobilenetv2  q_mobilenetv2_w1: graph and un-frozen arithmetic only (no frozen integer path yet, DESIGN.md section 2 row f3)
+  q_mobilenetv2  q_mobilenetv2_w1 (same module names as the reference; frozen, it runs on the integer engine too)
   bit_config   bit_config_dict(), get_bit_config(arch, scheme), stamp_bit_config(model, cfg)
   engine       compile_model(model, example) -> CompiledModel (one CUDA graph per GPU), all_gather_logits
   ops / _lib   the C ABI (include/hawq_b200.h) through ctypes
@@ -27,11 +27,11 @@ __version__ = "0.1.0"
 
 
 def build_synthetic_qresnet(arch, scheme, calib_batch=4, calib_seed=0, act_ranges=None):
-    """Seed-0 synthetic quantized ResNet (SURVEY.md §8d): float skeleton -> quantized graph -> bit config ->
-    calibration (one float forward on CPU, or ranges loaded like a checkpoint) -> frozen."""
+    """Seed-0 synthetic quantized ResNet or MobileNetV2 (``mobilenetv2_w1``) (SURVEY.md §8d): float skeleton -> quantized graph ->
+    bit config -> calibration (one float forward on CPU, or ranges loaded like a checkpoint) -> frozen."""
     import torch
-    from .synthetic import synthetic_batch, synthetic_float_resnet
-    net = synthetic_float_resnet(arch, 0)
+    from .synthetic import synthetic_batch, synthetic_float_mobilenetv2, synthetic_float_resnet
+    net = synthetic_float_mobilenetv2(0) if arch == "mobilenetv2_w1" else synthetic_float_resnet(arch, 0)
     q = quantize_arch_dict[arch](net)
     cfg = get_bit_config(arch, scheme)
     matched = stamp_bit_config(q, cfg)

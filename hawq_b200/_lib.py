@@ -67,6 +67,8 @@ SIGNATURES = {
     "hawq_linear_i8": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "hawq_stem_conv_i8": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp]),
     "hawq_stem_pool_i8": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _i32, _u32, _i32, _i32, _i32, _vp, _vp]),
+    "hawq_dwconv3x3": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "hawq_stem3x3_i8": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i32, _u32, _i32, _i32, _i32, _vp, _vp]),
     "hawq_maxpool_requant": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _i32, _u32, _i32, _i32, _i32, _vp, _vp]),
     "hawq_avgpool_requant": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _u32, _i32, _i32, _i32, _vp, _vp]),
     "hawq_quantize_input_f32": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _f32, _i32, _i32, _vp, _vp]),

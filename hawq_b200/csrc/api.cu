@@ -10,6 +10,7 @@
 #include "conv_igemm.cuh"
 #include "conv_tail.cuh"
 #include "elementwise.cuh"
+#include "mobilenet.cuh"
 #include "stem.cuh"
 
 using namespace hawq;
@@ -64,6 +65,7 @@ static int set_conv_attr() {
   constexpr int smem = ConvSmem<BN, A4>::TOTAL;
   int rc;
   if ((rc = set_smem_attr(conv_igemm_kernel<BN, A4, FAM_REQUANT>, smem)) || (rc = set_smem_attr(conv_igemm_kernel<BN, A4, FAM_RESIDUAL>, smem)) ||
+      (rc = set_smem_attr(conv_igemm_kernel<BN, A4, FAM_REQUANT_CAPPED>, smem)) ||
       (rc = set_smem_attr(conv_igemm_kernel<BN, A4, FAM_STORE>, smem)) ||
       (rc = set_smem_attr(conv_tail_kernel<A4, false>, TailSmem<A4, false>::TOTAL)) ||
       (rc = set_smem_attr(conv_tail_kernel<A4, true>, TailSmem<A4, true>::TOTAL)))
@@ -78,7 +80,8 @@ template <int BN, bool A4>
 static void launch_conv(const ConvParams& p, cudaStream_t s) {
   const int smem = ConvSmem<BN, A4>::TOTAL;
   const dim3 grid = conv_grid(p.M, p.Cout, BN);
-  if (p.mode == HAWQ_EPI_REQUANT) conv_igemm_kernel<BN, A4, FAM_REQUANT><<<grid, CONV_THREADS, smem, s>>>(p);
+  if (p.mode == HAWQ_EPI_REQUANT && p.relu == 2) conv_igemm_kernel<BN, A4, FAM_REQUANT_CAPPED><<<grid, CONV_THREADS, smem, s>>>(p);
+  else if (p.mode == HAWQ_EPI_REQUANT) conv_igemm_kernel<BN, A4, FAM_REQUANT><<<grid, CONV_THREADS, smem, s>>>(p);
   else if (p.mode == HAWQ_EPI_RESIDUAL) conv_igemm_kernel<BN, A4, FAM_RESIDUAL><<<grid, CONV_THREADS, smem, s>>>(p);
   else conv_igemm_kernel<BN, A4, FAM_STORE><<<grid, CONV_THREADS, smem, s>>>(p);
 }
@@ -350,6 +353,65 @@ int hawq_stem_conv_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int
   const int ctas = (int)(tiles < 4LL * h->sm_count ? tiles : 4LL * h->sm_count);
   stem_conv_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(x, (const uint32_t*)w, chan, N, H, W, Ho, Wo, clamp_lo, clamp_hi, out);
   return launch_check("stem_conv");
+}
+
+// MobileNetV2 depthwise 3x3 + case-0 requant (mobilenet.cuh); the caps of relu 2 come from chan[c].reserved (load_channel_block)
+int hawq_dwconv3x3(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_t C, int32_t stride, int32_t a_bits, const void* x,
+                   const int8_t* w, const hawq_chan* chan, int32_t relu, int32_t out_bits, int32_t clamp_lo, int32_t clamp_hi,
+                   void* out, void* stream) {
+  if (!h || !x || !w || !chan || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_dwconv3x3: null argument");
+  if (N < 1 || H < 1 || W < 1 || C < 1 || (stride != 1 && stride != 2)) return fail(HAWQ_ERR_BAD_ARG, "hawq_dwconv3x3: bad geometry");
+  if (C % DW_CB != 0) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: C (%d) must be a multiple of 16", C);
+  if (a_bits != 8 && a_bits != 4) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: a_bits must be 4 or 8");
+  if (out_bits != 8 && out_bits != 4) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: out_bits must be 4 or 8");
+  if (clamp_lo > clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_dwconv3x3: empty clamp range");
+  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  const long long pix = (long long)N * H * W;
+  if (pix > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: too many pixels");
+  const long long strips = (long long)N * ((Ho + DW_ROWS - 1) / DW_ROWS) * Wo;
+  const long long ctas = (strips + DW_THREADS - 1) / DW_THREADS * (C / DW_CB);
+  if (ctas > 0x7fffffffll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: more than 2^31 - 1 CTAs");
+  ConvParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = out; p.status = h->status;
+  p.N = N; p.H = H; p.W = W; p.Cin = C; p.Cout = C; p.KH = 3; p.KW = 3; p.stride = stride; p.pad = 1; p.Ho = Ho; p.Wo = Wo;
+  p.M = (int)((long long)N * Ho * Wo); p.K = 9;
+  p.mode = HAWQ_EPI_REQUANT; p.relu = relu; p.out_bits = out_bits; p.lo = clamp_lo; p.hi = clamp_hi;
+  set_bias_window(p, a_bits);
+  ++g_kernel_count[1];
+  if (a_bits == 8) dwconv3x3_kernel<false><<<(unsigned)ctas, DW_THREADS, 0, (cudaStream_t)stream>>>(p);
+  else dwconv3x3_kernel<true><<<(unsigned)ctas, DW_THREADS, 0, (cudaStream_t)stream>>>(p);
+  return launch_check("dwconv3x3");
+}
+
+// MobileNetV2 stem: 3x3 stride 2 pad 1, Cin 3 -> 64 stored channels, requant (+ ReLU6 caps), stream + optional low-bit copy
+int hawq_stem3x3_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_t* x, const int8_t* w, const hawq_chan* chan, int32_t relu,
+                    int32_t clamp_lo, int32_t clamp_hi, int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
+                    int32_t low_lo, int32_t low_hi, void* out_low, void* stream) {
+  if (!h || !x || !w || !chan || !y) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: null argument");
+  if (N < 1 || H < 1 || W < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: bad geometry");
+  if (clamp_lo > clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: empty clamp range");
+  if (y_bits == 16 && (clamp_lo < -32768 || clamp_hi > 32767)) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: clamp must fit int16");
+  if ((y_bits != 16 && y_bits != 32) || (low_bits != 0 && low_bits != 4 && low_bits != 8) || (low_bits && !out_low))
+    return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: bad output description");
+  if (low_bits) { int rc = check_me(low_m, low_e, "hawq_stem3x3_i8"); if (rc) return rc; }
+  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+  if ((long long)N * H * W > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem3x3_i8: too many pixels");
+  const long long ctas = (long long)N * Ho * ((Wo + STEM3_PX - 1) / STEM3_PX);
+  if (ctas > 0x7fffffffll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem3x3_i8: more than 2^31 - 1 CTAs");
+  ConvParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = y; p.out_low = out_low; p.status = h->status;
+  p.N = N; p.H = H; p.W = W; p.Cin = 3; p.Cout = 64; p.KH = 3; p.KW = 3; p.stride = 2; p.pad = 1; p.Ho = Ho; p.Wo = Wo;
+  p.M = (int)((long long)N * Ho * Wo); p.K = 27;
+  p.mode = HAWQ_EPI_REQUANT; p.relu = relu; p.lo = clamp_lo; p.hi = clamp_hi; p.y_bits = y_bits;
+  p.low_bits = low_bits; p.low_m = low_m; p.low_e = low_e; p.low_lo = low_lo; p.low_hi = low_hi;
+  // a low-bit ratio > 1 takes the CTA to the exact requantisation (load_channel_block)
+  p.scalar_over_one = p.scalar_unchecked = low_bits != 0 && !dyadic_is_fast(low_m, low_e);
+  set_bias_window(p, 8);
+  ++g_kernel_count[2];
+  stem3x3_kernel<<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(p);
+  return launch_check("stem3x3");
 }
 
 int hawq_stem_pool_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_t* x, const int8_t* w256, const hawq_chan* chan,

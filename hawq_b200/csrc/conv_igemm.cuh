@@ -109,8 +109,9 @@ __device__ __forceinline__ int swz(int row, int ch) {
 }
 
 // Epilogue family of an instantiation (FAM): REQUANT to 4/8/16/32 bits, RESIDUAL, STORE (RAW_I32 and
-// DEQUANT_F32, no requantisation).  A kernel carries its own family's body only.
-constexpr int FAM_REQUANT = 0, FAM_RESIDUAL = 1, FAM_STORE = 2;
+// DEQUANT_F32, no requantisation), and REQUANT with per-channel ReLU6 caps (relu 2).  A kernel carries its own family's body only;
+// the capped REQUANT has its own copy so that the uncapped one (relu 0 / 1) keeps its code and registers.
+constexpr int FAM_REQUANT = 0, FAM_RESIDUAL = 1, FAM_STORE = 2, FAM_REQUANT_CAPPED = 3;
 
 // One requantised term q = RHE(value * m / 2^e) of an epilogue, in one of two implementations; the kernel picks one per CTA.
 // Operands are built by acc_bias (acc + bias of a channel), of_i32 and of_u16; term() takes the ratio both as M = m * 2^-e and as
@@ -168,13 +169,15 @@ struct RqPolicy {
 };
 
 // Loads the channel block n0 ... n0 + BN - 1 (and, for a res_kind 1 RESIDUAL, its res_chan) into shared memory and returns the
-// CTA's policy.  Every thread of the CTA must call it (three __syncthreads_or).
-template <int BN, bool RESIDUAL>
+// CTA's policy.  CAPS: .reserved becomes the channel's upper clamp, min(hi, reserved) under relu 2 (ReLU6), else hi.  Every thread
+// of the CTA must call it (three __syncthreads_or).
+template <int BN, bool RESIDUAL, bool CAPS = false>
 __device__ RqPolicy load_channel_block(const ConvParams& p, int n0, const ChanSmem<BN>& cs) {
   int over_one = p.scalar_over_one, unchecked = p.scalar_unchecked, bias_out = 0;
   const int tid = threadIdx.x;
   if (tid < BN) {
-    const hawq_chan c = p.chan[n0 + tid];
+    hawq_chan c = p.chan[n0 + tid];
+    if (CAPS) c.reserved = p.relu == 2 ? min(p.hi, c.reserved) : p.hi;
     cs.chan[tid] = c;
     cs.M[tid] = dyadic_to_double(c.m, c.e);
     cs.Cb[tid] = 4503601774854144.0 - (double)c.bias;   // exact: folds the bias add into the int -> double conversion
@@ -303,7 +306,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   const int m0 = (int)(blockIdx.x / nblk) * BM;
   const int n0 = (int)(blockIdx.x % nblk) * BN;
 
-  const RqPolicy pol = load_channel_block<BN, FAM == FAM_RESIDUAL>(p, n0, cs);
+  constexpr bool REQ = FAM == FAM_REQUANT || FAM == FAM_REQUANT_CAPPED;
+  const RqPolicy pol = load_channel_block<BN, FAM == FAM_RESIDUAL, FAM == FAM_REQUANT_CAPPED>(p, n0, cs);
 
   int32_t acc[NACC];
 
@@ -440,8 +444,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
 
   // ------------------------------------------------------------------------------------------------ epilogue
   uint8_t* sOut = smem;
-  const bool stage_low = (FAM == FAM_REQUANT && p.out_bits <= 8) || (FAM == FAM_RESIDUAL && p.low_bits != 0);
-  const int stage_bits = (FAM == FAM_REQUANT) ? p.out_bits : p.low_bits;
+  const bool stage_low = (REQ && p.out_bits <= 8) || (FAM == FAM_RESIDUAL && p.low_bits != 0);
+  const int stage_bits = REQ ? p.out_bits : p.low_bits;
 
   auto put_low = [&](int row, int col, int q0, int q1) { stage_low_pair(sOut, S::OUT_PITCH, row, col, q0, q1); };
   // a pair of the new residual stream, staged or stored directly
@@ -458,21 +462,23 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   // 4/8-bit outputs (staged) and 16/32-bit outputs (stored directly), so that no store branch splits the unrolled loop and the
   // terms' FP64 latencies overlap
   auto epilogue = [&](auto rq, auto low_out) {
-    if constexpr (FAM == FAM_REQUANT) {
-      // clamp(RHE((acc + bias) * ratio)), ReLU folded into the lower clamp bound (both implementations are monotone with RHE(0) = 0)
+    if constexpr (REQ) {
+      // clamp(RHE((acc + bias) * ratio)), ReLU folded into the lower clamp bound (both implementations are monotone with RHE(0) = 0);
+      // capped: the channel's upper clamp from load_channel_block (clamp_hi, or its ReLU6 cap)
       const int lo = p.relu ? min(max(p.lo, 0), p.hi) : p.lo;
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
         const int col = ni * 8 + 2 * t;
-        const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);   // bias, m, e
+        const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);   // bias, m, e (capped: upper clamp)
         const int4 c1 = *reinterpret_cast<const int4*>(&sChan[col + 1]);
         const double2 M = *reinterpret_cast<const double2*>(&sM[col]);
         const double2 Cb = *reinterpret_cast<const double2*>(&sCb[col]);
+        const int hi0 = FAM == FAM_REQUANT_CAPPED ? c0.w : p.hi, hi1 = FAM == FAM_REQUANT_CAPPED ? c1.w : p.hi;
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
           const int row = warp * 16 + hf * 8 + g;
-          const int q0 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2], Cb.x, c0.x), M.x, c0.y, c0.z, false), lo, p.hi);
-          const int q1 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2 + 1], Cb.y, c1.x), M.y, c1.y, c1.z, false), lo, p.hi);
+          const int q0 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2], Cb.x, c0.x), M.x, c0.y, c0.z, false), lo, hi0);
+          const int q1 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2 + 1], Cb.y, c1.x), M.y, c1.y, c1.z, false), lo, hi1);
           if constexpr (decltype(low_out)::value) {
             put_low(row, col, q0, q1);
           } else if (m0 + row < p.M) {
@@ -549,7 +555,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
     }
   } else {
     auto run = [&](auto low_out) { with_rq<FAM == FAM_RESIDUAL>(pol, p, [&](auto rq) { epilogue(rq, low_out); }); };
-    if (FAM == FAM_REQUANT && p.out_bits <= 8) run(std::true_type{});
+    if (REQ && p.out_bits <= 8) run(std::true_type{});
     else run(std::false_type{});
   }
 
@@ -557,7 +563,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   if (y_staged)   // coalesced copy-out of the new residual stream tile
     copy_out_rows(sY, y_pitch, reinterpret_cast<uint8_t*>(p.out) + (size_t)n0 * y_es, (size_t)p.Cout * y_es, BN * y_es, m0, p.M);
   if (stage_low)
-    copy_out_low<BN>(sOut, S::OUT_PITCH, reinterpret_cast<uint8_t*>(FAM == FAM_REQUANT ? p.out : p.out_low), stage_bits, m0, n0, p.M, p.Cout);
+    copy_out_low<BN>(sOut, S::OUT_PITCH, reinterpret_cast<uint8_t*>(REQ ? p.out : p.out_low), stage_bits, m0, n0, p.M, p.Cout);
 }
 
 }  // namespace hawq

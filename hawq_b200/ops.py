@@ -82,14 +82,21 @@ def conv_work(desc, ep):
     return macs, b
 
 
-def make_chan(bias, m, e):
-    """hawq_chan[C] as an int32 [C,4] CPU tensor (m stored by bit pattern)."""
+def make_chan(bias, m, e, cap=None):
+    """hawq_chan[C] as an int32 [C,4] CPU tensor (m stored by bit pattern; `cap`: the ReLU6 output caps of relu 2, in reserved)."""
     c = len(bias)
     a = np.zeros((c, 4), dtype=np.int32)
     a[:, 0] = np.asarray(bias, dtype=np.int64).astype(np.int32)
     a[:, 1] = np.asarray(m, dtype=np.uint64).astype(np.uint32).view(np.int32)
     a[:, 2] = np.asarray(e, dtype=np.int32)
+    if cap is not None:
+        a[:, 3] = np.asarray(cap, dtype=np.int64).astype(np.int32)
     return torch.from_numpy(a)
+
+
+def rhe_requant_host(v, m, e):
+    """RHE(v * m / 2^e) of one int32 value, exact (the library's host helper, the routine the kernels inline)."""
+    return int(_lib.load().hawq_rhe_requant_host(int(v), int(m), int(e)))
 
 
 def conv_desc(N, H, W, Cin, Cout, kh, kw, stride, pad, a_bits, w_layout=0):
@@ -132,9 +139,43 @@ def ratio_flags(*pairs):
     return 0
 
 
-def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None, out_low=None):
+def _with_logical(work, logical_work, logical):
+    """work() -> (MACs, bytes) at the stored (padded) channel counts; with `logical` (the model's channel counts) a third entry,
+    the bytes at the logical counts, so that the cost of padding is visible."""
+    if logical is None:
+        return work
+    return lambda: tuple(work()) + (logical_work(*logical)[1],)
+
+
+def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None, out_low=None, logical=None):
+    """`logical`: (Cin, Cout) of the model when the descriptor's are padded (timer work only)."""
+    def logical_work(cin, cout):
+        d = hawq_conv_desc(*[getattr(desc, f) for f, _ in hawq_conv_desc._fields_])
+        d.Cin, d.Cout = cin, cout
+        return conv_work(d, ep)
     _launch(x, "hawq_conv2d", C.byref(desc), C.byref(ep), _p(x), _p(w), _p(chan), _p(res), _p(res_chan), _p(fscale), _p(out),
-            _p(out_low), label="conv_igemm", work=lambda: conv_work(desc, ep))
+            _p(out_low), label="conv_igemm", work=_with_logical(lambda: conv_work(desc, ep), logical_work, logical))
+
+
+def dwconv3x3(x, n, hh, ww, c, stride, a_bits, w, chan, relu, out_bits, clamp, out, logical=None):
+    """Depthwise 3x3 pad 1 + case-0 requant (hawq_dwconv3x3); `logical`: (C,) of the model when c is padded (timer work only)."""
+    ho, wo = (hh - 1) // stride + 1, (ww - 1) // stride + 1
+
+    def work(cc):
+        return n * ho * wo * cc * 9, n * hh * ww * cc * a_bits // 8 + 9 * cc + 16 * cc + n * ho * wo * cc * out_bits // 8
+    _launch(x, "hawq_dwconv3x3", n, hh, ww, c, stride, a_bits, _p(x), _p(w), _p(chan), int(relu), out_bits, clamp[0], clamp[1], _p(out),
+            label="dwconv3x3", work=_with_logical(lambda: work(c), work, logical))
+
+
+def stem3x3(x, w, chan, relu, clamp, n, hh, ww, y_bits, y, low_bits, low_me, low_clamp, out_low, logical=None):
+    """MobileNetV2 stem: 3x3/2 convolution of 3 channels -> 64 stored channels + requant (hawq_stem3x3_i8), optional low-bit copy;
+    `logical`: (Cout,) of the model (timer work only)."""
+    ho, wo = (hh - 1) // 2 + 1, (ww - 1) // 2 + 1
+
+    def work(cc):
+        return n * ho * wo * cc * 27, n * hh * ww * 3 + cc * 36 + 16 * cc + n * ho * wo * cc * (y_bits + low_bits) // 8
+    _launch(x, "hawq_stem3x3_i8", n, hh, ww, _p(x), _p(w), _p(chan), int(relu), clamp[0], clamp[1], y_bits, _p(y), low_bits, low_me[0],
+            low_me[1], low_clamp[0], low_clamp[1], _p(out_low), label="stem3x3", work=_with_logical(lambda: work(64), work, logical))
 
 
 def conv2d_dual(x, desc, ep, w, chan, desc2, x2, w2, chan2, out=None, out_low=None):

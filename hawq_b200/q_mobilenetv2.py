@@ -8,11 +8,11 @@ bit configs, ``bit_config.py:3602-4202``, and checkpoints key identically):
   net:   quant_input -> init_block 3x3/2 + ReLU6 -> quant_act_int32 -> units -> quant_act_before_final_block -> final_block 1x1 +
          ReLU6 -> quant_act_int32_final -> final_pool -> quant_act_output -> output (QuantConv2d 1x1) -> logits
 
-STATUS (DESIGN.md section 2, row f3): the graph runs un-frozen (calibration / evaluation of the fake-quant arithmetic, same numbers
-as the reference, tests/test_mobilenetv2_cpu.py) and the oracle for the frozen integers is pinned to the reference
-(oracle/fakequant.py FakeQuantMobileNetV2, tests/golden/net_mobilenetv2_w1_*.npz).  The frozen integer path is NOT built: it
-needs a depthwise kernel, ReLU6 as a per-channel output clamp and a signed residual stream; a frozen forward raises
-NotImplementedError from the convolution planner instead of computing something else.
+Un-frozen, the graph runs the reference's fake-quant arithmetic (calibration; tests/test_mobilenetv2_cpu.py).  Frozen, it runs on
+the integer engine (qtensor.py, DESIGN.md section 2 row f3): the stem and the depthwise layers on their own kernels
+(hawq_stem3x3_i8, hawq_dwconv3x3), every 1x1 layer on the convolution kernel with channels zero-padded to multiples of 64, ReLU6
+as a per-channel output clamp of the consuming QuantAct, the signed 16-bit stream stored as int32, and the 1x1 classifier as
+fp32 logits; ``compile_model`` captures it in one CUDA graph like the ResNets.
 """
 import torch.nn as nn
 
@@ -98,9 +98,6 @@ class Q_MobileNetV2(nn.Module):
                 yield getattr(stage, "unit%d" % ui)
 
     def forward(self, x):
-        if self.init_block.fix_flag:
-            raise NotImplementedError("hawq_b200 has no frozen (integer) path for MobileNetV2: the engine lacks a depthwise kernel, the ReLU6 "
-                                      "clamp and a signed residual stream (DESIGN.md section 2, row f3). Un-frozen forwards work.")
         relu6 = self.activatition_func
         x, a_sf = self.quant_input(x)
         x, w_sf = self.init_block(x, a_sf)

@@ -10,8 +10,14 @@ been launched yet.  Pending producers are how the reference's module-by-module g
 consuming ``QuantAct`` is reached, with that activation's dyadic requantisation (and, for residual sums, the NEXT
 unit's low-bit activation) folded into the kernel epilogue.
 
-``nn.ReLU``, ``nn.MaxPool2d``, ``+``, ``.view`` on an ``IntActivation`` are intercepted through
+``nn.ReLU``, ``nn.ReLU6``, ``nn.MaxPool2d``, ``+``, ``.view`` on an ``IntActivation`` are intercepted through
 ``__torch_function__`` and recorded on the node; anything else is not an integer-path operation and raises.
+
+Channel padding: a convolution output or stream whose channel count is not a multiple of 64 (MobileNetV2's 16 / 24 / 32 / 96 /
+144 ... channels) is stored zero-padded to the next multiple of 64 (``stored_channels``), so every 1x1 layer runs on the
+convolution kernel unchanged.  Padded weight rows and columns, biases and multipliers are 0, so every padded channel is exactly 0
+in every tensor (RHE(0) = 0, and a case-1 sum of zeros is 0).  ``Node.shape`` keeps the logical shape, ``Node.cs`` the stored
+channel count that every descriptor uses.
 """
 import contextlib
 import copy
@@ -80,18 +86,34 @@ class Node:
          'stem'     pending stem conv + pool + 16-bit requant by QuantAct `act` (+relu)
          'avgpool'  pending integer average pool of src
     """
-    __slots__ = ("kind", "shape", "data", "bits", "signed", "mod", "src", "a_sf", "relu", "pool", "a", "b", "act", "args")
+    __slots__ = ("kind", "shape", "cs", "data", "bits", "signed", "mod", "src", "a_sf", "relu", "relu6", "pool", "a", "b", "act", "args")
 
     def __init__(self, kind, shape, **kw):
         self.kind, self.shape = kind, tuple(shape)
+        self.cs = self.shape[1]          # stored channels: an input handed in by the caller is not padded
         self.data = self.mod = self.src = self.a_sf = self.a = self.b = self.act = self.args = self.pool = None
-        self.bits, self.signed, self.relu = 0, True, False
+        self.bits, self.signed, self.relu, self.relu6 = 0, True, False, False
         for k, v in kw.items():
             setattr(self, k, v)
 
     def become_int(self, data, bits, signed):
         self.kind, self.data, self.bits, self.signed = "int", data, bits, signed
+        self.cs = stored_channels(self.shape[1])
         self.mod = self.src = self.a = self.b = self.act = self.args = None
+
+
+def stored_channels(c):
+    """Channels of a kernel-written tensor with c logical channels in HBM: zero-padded to a multiple of 64."""
+    return -(-c // 64) * 64
+
+
+def _stored_shape(shape):
+    return (shape[0], stored_channels(shape[1])) + tuple(shape[2:])
+
+
+def _new_int(device, shape, bits, signed):
+    """Node 'int' with fresh storage for a kernel output of logical shape `shape` (channels padded, stored_channels)."""
+    return Node("int", shape, data=_alloc(device, _stored_shape(shape), bits), bits=bits, signed=signed, cs=stored_channels(shape[1]))
 
 
 class IntActivation(torch.Tensor):
@@ -112,6 +134,8 @@ class IntActivation(torch.Tensor):
         name = getattr(func, "__name__", str(func))
         if name in ("relu", "relu_"):
             return _relu(args[0])
+        if name in ("hardtanh", "hardtanh_", "relu6", "relu6_"):
+            return _relu6(name, *args, **kwargs)
         if name in ("max_pool2d", "_max_pool2d", "max_pool2d_with_indices"):
             return _max_pool(*args, **kwargs)
         if name in ("add", "__add__", "__radd__", "__iadd__", "add_"):
@@ -123,7 +147,7 @@ class IntActivation(torch.Tensor):
                 return func(*args, **kwargs)
         raise NotImplementedError(
             "torch op %r on an IntActivation is not part of the HAWQ integer path (supported between frozen "
-            "modules: ReLU, MaxPool2d(3,2,1) after the stem, +, view/flatten). Use .dequantize() for a float tensor." % name)
+            "modules: ReLU, ReLU6, MaxPool2d(3,2,1) after the stem, +, view/flatten). Use .dequantize() for a float tensor." % name)
 
     @classmethod
     def __torch_dispatch__(cls, func, types, args=(), kwargs=None):
@@ -136,15 +160,16 @@ class IntActivation(torch.Tensor):
         shp = self.node.shape
         nb, c = shp[0], shp[1]
         hh, ww = (shp[2], shp[3]) if len(shp) == 4 else (1, 1)
-        out = torch.empty((nb, c, hh, ww), dtype=torch.float32, device=self.device)
-        ops.dequant(n.data, nb, hh, ww, c, n.bits, n.signed, s, out)
-        return out.view(*self.shape)
+        out = torch.empty((nb, n.cs, hh, ww), dtype=torch.float32, device=self.device)
+        ops.dequant(n.data, nb, hh, ww, n.cs, n.bits, n.signed, s, out)
+        return out[:, :c].contiguous().view(*self.shape)
 
     def int_tensor(self):
-        """Concrete integers as an int32 tensor in logical (NCHW / NC) order — for tests and debugging."""
+        """Concrete integers as an int32 tensor in logical (NCHW / NC) order, padded channels dropped — for tests and debugging."""
         n = materialize(self.node, self.device)
-        return unpack_to_int32(n).view(self.node.shape[0], *([self.node.shape[2], self.node.shape[3]] if len(self.node.shape) == 4 else []),
-                                       self.node.shape[1]).permute(*((0, 3, 1, 2) if len(self.node.shape) == 4 else (0, 1))).contiguous()
+        shp = self.node.shape
+        v = unpack_to_int32(n).view(shp[0], *([shp[2], shp[3]] if len(shp) == 4 else []), n.cs)[..., :shp[1]]
+        return v.permute(*((0, 3, 1, 2) if len(shp) == 4 else (0, 1))).contiguous()
 
 
 def unpack_to_int32(n):
@@ -274,38 +299,100 @@ def _conv_cache(mod, a_sf, a_bits, device):
 
 
 def _conv_params(mod, a_sf, a_bits, device):
+    """kind: 'conv' (conv_igemm: OHWI, channels padded to stored_channels), 'stem' (ResNet 7x7/2 stem), 'stem3' (MobileNetV2 3x3/2
+    stem, hawq_stem3x3_i8: [64][3][3][4]) or 'dw' (depthwise 3x3, hawq_dwconv3x3: [3][3][C stored]).  cin / cout are the stored
+    channel counts, cout_l the logical one."""
     conv = mod.conv
     src_dev = conv.weight.device
     w_sf, w_int, b_int, _ = mod.integer_params(a_sf.to(src_dev))
     w_sf = w_sf.detach().to("cpu", torch.float32)
-    cout, cin, kh, kw = w_int.shape
-    if conv.groups != 1 or conv.dilation[0] != 1 or conv.dilation[1] != 1 or kh != kw or conv.stride[0] != conv.stride[1]:
-        raise NotImplementedError("hawq_b200 convolutions: groups=1, dilation=1, square kernels/strides only")
+    cout, cin_g, kh, kw = w_int.shape
+    groups = conv.groups
+    cin = cin_g * groups
+    dw = groups != 1 and groups == cin == cout and kh == 3 and cin_g == 1
+    if (groups != 1 and not dw) or conv.dilation[0] != 1 or conv.dilation[1] != 1 or kh != kw or conv.stride[0] != conv.stride[1]:
+        raise NotImplementedError("hawq_b200 convolutions: groups=1 or depthwise 3x3, dilation=1, square kernels/strides only")
     w = w_int.detach().to("cpu").permute(0, 2, 3, 1).contiguous().to(torch.int8)      # OHWI
-    bias = (b_int.detach().to("cpu").to(torch.int64).numpy() if b_int is not None else np.zeros(cout, dtype=np.int64))
-    stem = (cin == 3 and kh == 7 and conv.stride[0] == 2 and conv.padding[0] == 3 and cout == 64)
-    if stem:
+    cin_s, cout_s = stored_channels(cin), stored_channels(cout)
+    bias = np.zeros(cout_s, dtype=np.int64)
+    if b_int is not None:
+        bias[:cout] = b_int.detach().to("cpu").to(torch.int64).numpy()
+    kind = "conv"
+    if cin == 3 and kh == 7 and conv.stride[0] == 2 and conv.padding[0] == 3 and cout == 64:
+        kind = "stem"
         wp = torch.zeros((cout, 8, 8, 4), dtype=torch.int8)       # kernel rows 7 -> 8, taps 7 -> 8, channels 3 -> 4 (zeros)
         wp[:, :7, :7, :3] = w
         w = wp[:, :7].contiguous()                                # stem kernel layout: K = 224
+        cin_s = 3
+    elif cin == 3 and kh == 3 and conv.stride[0] == 2 and conv.padding[0] == 1 and cout <= 64:
+        kind = "stem3"
+        wp = torch.zeros((64, 3, 3, 4), dtype=torch.int8)         # output channels -> 64, input channels 3 -> 4 (zeros)
+        wp[:cout, :, :, :3] = w
+        w, cin_s = wp, 3
+    elif dw:
+        if conv.padding[0] != 1 or conv.stride[0] not in (1, 2):
+            raise NotImplementedError("hawq_b200 depthwise convolutions: 3x3, pad 1, stride 1 or 2")
+        kind = "dw"
+        wp = torch.zeros((3, 3, cout_s), dtype=torch.int8)        # channel-minor: one 16-byte load holds 16 channels of a tap
+        wp[:, :, :cout] = w[:, :, :, 0].permute(1, 2, 0)
+        w = wp
     else:
-        if cin % 64 != 0 or cout % 64 != 0:
-            raise NotImplementedError("hawq_b200 convolutions need Cin and Cout multiples of 64 (got %d, %d)" % (cin, cout))
+        wp = torch.zeros((cout_s, kh, kw, cin_s), dtype=torch.int8)
+        wp[:cout, :, :, :cin] = w
+        w = wp
         if a_bits == 4:
             ops.permute_weights_for_i4(w)
-    tiled = (not stem) and torch.device(device).type == "cuda"
-    return dict(w=ops.upload_weights(w, device) if tiled else w.to(device), w_layout=1 if tiled else 0, w_sf=w_sf, bias=bias, cout=cout, cin=cin, k=kh, stride=conv.stride[0],
-                pad=conv.padding[0], stem=stem, chan={})
+    tiled = kind == "conv" and torch.device(device).type == "cuda"
+    return dict(w=ops.upload_weights(w, device) if tiled else w.to(device), w_layout=1 if tiled else 0, w_sf=w_sf, bias=bias,
+                cout=cout_s if kind != "stem3" else 64, cin=cin_s, cout_l=cout, k=kh, stride=conv.stride[0], pad=conv.padding[0],
+                stem=kind == "stem", kind=kind, chan={})
 
 
-def _chan_tensor(ent, tag, m, e, device):
+def _pad_me(m, e, c):
+    """(m, e) lists of the logical channels (or one scalar pair) -> c stored channels; padded channels get m = 0."""
+    if len(m) == 1 or len(m) == c:
+        return list(m), list(e)
+    return list(m) + [0] * (c - len(m)), list(e) + [1] * (c - len(e))
+
+
+def _chan_tensor(ent, tag, m, e, device, caps=None):
+    """Cached hawq_chan table of plan `ent`; `caps`: a function giving the ReLU6 caps (computed on a cache miss only)."""
     t = ent["chan"].get(tag)
     if t is None:
-        t = ent["chan"][tag] = ops.make_chan(ent["bias"], m, e).to(device)
+        m, e = _pad_me(m, e, len(ent["bias"]))
+        t = ent["chan"][tag] = ops.make_chan(ent["bias"], m, e, caps() if caps else None).to(device)
     return t
 
 
+def _relu6_caps(n, ent, m, e, hi):
+    """Per-channel output caps of ReLU6 (hawq_chan.reserved with relu 2): ReLU6 caps the accumulator at
+    C_c = round_f32(6 / a_sf / w_sf_c) (the reference clamps the fp32 value acc * a_sf * w_sf_c at 6 and its QuantAct recovers
+    round(z / a_sf / w_sf_c)); the requantisation is monotone, so the output cap is RHE(C_c * m_c / 2^e_c).  A cap C_c >= 2^31
+    can never bind: hi.  Padded channels: hi."""
+    cl = ent["cout_l"]
+    acc_cap = np.broadcast_to(np.rint(np.float32(6.0) / _cpu_f32(n.a_sf).numpy()[0] / _cpu_f32(ent["w_sf"]).numpy()), (cl,))
+    mm, ee = (m, e) if len(m) == cl else (list(m) * cl, list(e) * cl)
+    caps = [min(hi, ops.rhe_requant_host(int(c), mm[i], ee[i])) if c < 2 ** 31 else hi for i, c in enumerate(acc_cap)]
+    return caps + [hi] * (len(ent["bias"]) - cl)
+
+
 # ------------------------------------------------------------------------------------------------ lazy ops
+def _relu6(name, x, *args, **kw):
+    """nn.ReLU6 (F.hardtanh(x, 0, 6)) or F.relu6 on a pending convolution: recorded as `relu6`, applied by the consuming QuantAct
+    as a per-channel clamp (_relu6_caps)."""
+    if name.startswith("hardtanh"):
+        pos = dict(zip(("min_val", "max_val"), args))
+        lo, hi = kw.get("min_val", pos.get("min_val", -1.0)), kw.get("max_val", pos.get("max_val", 1.0))
+        if float(lo) != 0.0 or float(hi) != 6.0:
+            raise NotImplementedError("hardtanh(%s, %s) on an IntActivation: only ReLU6 = hardtanh(0, 6) is part of the integer path" % (lo, hi))
+    n = x.node
+    if n.kind != "conv" or n.pool is not None:
+        raise NotImplementedError("ReLU6 on an IntActivation must follow a convolution directly (got a %s)" % n.kind)
+    m = copy.copy(n)
+    m.relu = m.relu6 = True
+    return IntActivation(m, x.device, x.shape)
+
+
 def _relu(x):
     n = x.node
     if n.kind in ("conv", "residual", "stem"):
@@ -368,6 +455,10 @@ def _desc(n, ent):
 
 
 def _launch_conv(n, ent, ep, chan, **kw):
+    if n.src.cs != ent["cin"]:
+        raise RuntimeError("convolution input has %d stored channels, its weights %d" % (n.src.cs, ent["cin"]))
+    if (n.src.shape[1], n.shape[1]) != (ent["cin"], ent["cout"]):      # padded channels: the timer also counts the logical bytes
+        kw["logical"] = (n.src.shape[1], n.shape[1])
     ops.conv2d(n.src.data, _desc(n, ent), ep, ent["w"], chan, **kw)
 
 
@@ -383,23 +474,34 @@ def _conv_case0(n, act, device):
     """conv [+ReLU] -> QuantAct case 0, one kernel."""
     _check_src(n)
     ent = _conv_cache(n.mod, n.a_sf, n.src.bits, device)
-    if ent["stem"]:
-        raise NotImplementedError("the stem convolution is only supported as conv -> MaxPool2d(3,2,1) -> 16-bit QuantAct")
+    if ent["kind"] in ("stem", "stem3"):
+        raise NotImplementedError("the stem convolution is only supported as conv -> MaxPool2d(3,2,1) -> 16-bit QuantAct (ResNet) "
+                                  "or conv -> ReLU6 -> 16-bit QuantAct (MobileNetV2)")
     m, e = _dyadic(act, n.a_sf, ent["w_sf"], "case0")
-    chan = _chan_tensor(ent, _act_tag("c0", act), m, e, device)
-    bits = _store_bits(act)
     lo, hi = _act_clamp(act)
-    out = _alloc(device, n.shape, bits)
-    ep = ops.epilogue(EPI_REQUANT, relu=n.relu, out_bits=bits, clamp=(lo, hi),
-                      flags=_ratio_flags((m, e)))
-    _launch_conv(n, ent, ep, chan, out=out)
-    return Node("int", n.shape, data=out, bits=bits, signed=_store_signed(act))
+    caps = (lambda: _relu6_caps(n, ent, m, e, hi)) if n.relu6 else None
+    chan = _chan_tensor(ent, _act_tag("c0r6" if n.relu6 else "c0", act), m, e, device, caps)
+    bits = _store_bits(act)
+    if bits == 16 and not n.relu:
+        bits = 32        # a signed 16-bit stream (MobileNetV2's quant_act_int32): 16-bit operands are read as uint16, so int32
+    out = _new_int(device, n.shape, bits, _store_signed(act))
+    relu = 2 if n.relu6 else n.relu
+    if ent["kind"] == "dw":
+        if n.src.cs != ent["cout"]:
+            raise RuntimeError("depthwise input has %d stored channels, its weights %d" % (n.src.cs, ent["cout"]))
+        nb, _, hh, ww = n.src.shape
+        ops.dwconv3x3(n.src.data, nb, hh, ww, ent["cout"], ent["stride"], n.src.bits, ent["w"], chan, relu, bits, (lo, hi), out.data,
+                      logical=(n.shape[1],))
+        return out
+    ep = ops.epilogue(EPI_REQUANT, relu=relu, out_bits=bits, clamp=(lo, hi), flags=_ratio_flags((m, e)))
+    _launch_conv(n, ent, ep, chan, out=out.data)
+    return out
 
 
 def _conv_raw(n, ent, device):
     """identity-branch conv: int32 accumulator + bias."""
     chan = _chan_tensor(ent, "raw", [0] * ent["cout"], [1] * ent["cout"], device)
-    out = _alloc(device, n.shape, 32)
+    out = _alloc(device, _stored_shape(n.shape), 32)
     _launch_conv(n, ent, ops.epilogue(EPI_RAW_I32, flags=_ratio_flags()), chan, out=out)
     return out
 
@@ -412,7 +514,7 @@ def _low_out(low_act, act, shape, device):
     _frozen_scale(low_act)                 # refreshes low_act's scale, which _dyadic reads
     lm, le = _dyadic(low_act, _frozen_scale(act), _ones(), "case0")
     bits = _store_bits(low_act)
-    node = Node("int", shape, data=_alloc(device, shape, bits), bits=bits, signed=_store_signed(low_act))
+    node = _new_int(device, shape, bits, _store_signed(low_act))
     return bits, (lm[0], le[0]), _act_clamp(low_act), node
 
 
@@ -440,8 +542,8 @@ def _launch_residual(r, low_act, device):
         res, res_chan = ident.data, None
         res_kind, res_bits, res_me = 0, ident.bits, (m1[0], e1[0])
         id_pair = res_me
-    y_bits = config.residual_bits if r.relu else 32
-    y = _alloc(device, r.shape, y_bits)
+    y_bits = config.residual_bits if r.relu else 32      # without ReLU (MobileNetV2) the stream is signed: int32
+    y = _alloc(device, _stored_shape(r.shape), y_bits)
     low_bits, low_me, low_clamp, low = _low_out(low_act, act, r.shape, device)
     ep = ops.epilogue(EPI_RESIDUAL, relu=r.relu, res_kind=res_kind, res_bits=res_bits, res_me=res_me, y_bits=y_bits,
                       low_bits=low_bits, low_me=low_me, low_clamp=low_clamp, flags=_ratio_flags((m2, e2), id_pair, low_me))
@@ -467,14 +569,28 @@ def _launch_residual(r, low_act, device):
 
 
 def _launch_stem(st, low_act, device):
-    """'stem' node: 7x7 conv (+bias, 16-bit requant, ReLU) -> int16, then max-pool -> residual stream (+ low-bit copy)."""
+    """'stem' node: 7x7 conv (+bias, 16-bit requant, ReLU) -> int16, then max-pool -> residual stream (+ low-bit copy); or the
+    MobileNetV2 stem, 3x3/2 conv (+bias, ReLU6, 16-bit requant) -> stream (+ low-bit copy) in one kernel."""
     conv, act = st.a, st.act
     src = conv.src
     if src.kind != "int" or src.bits != 8 or not src.signed:
         raise NotImplementedError("stem input must be signed int8")
+    ent = _conv_cache(conv.mod, conv.a_sf, 8, device)
+    if ent["kind"] == "stem3":
+        m, e = _dyadic(act, conv.a_sf, ent["w_sf"], "case0")
+        lo, hi = _act_clamp(act)
+        caps = (lambda: _relu6_caps(conv, ent, m, e, hi)) if conv.relu6 else None
+        chan = _chan_tensor(ent, _act_tag("c0r6" if conv.relu6 else "c0", act), m, e, device, caps)
+        y_bits = config.residual_bits if conv.relu else 32
+        y = _alloc(device, _stored_shape(st.shape), y_bits)
+        low_bits, low_me, low_clamp, low = _low_out(low_act, act, st.shape, device)
+        nb, _, hh, ww = src.shape
+        ops.stem3x3(src.data, ent["w"], chan, 2 if conv.relu6 else conv.relu, (lo, hi), nb, hh, ww, y_bits, y, low_bits, low_me,
+                    low_clamp, low.data if low is not None else None, logical=(st.shape[1],))
+        st.become_int(y, y_bits, signed=(y_bits == 32))
+        return low
     if not st.relu:
         raise NotImplementedError("the fused stem expects the reference order conv -> pool -> QuantAct(16) -> ReLU")
-    ent = _conv_cache(conv.mod, conv.a_sf, 8, device)
     m, e = _dyadic(act, conv.a_sf, ent["w_sf"], "case0")
     chan = _chan_tensor(ent, _act_tag("c0", act), m, e, device)
     nb, _, hh, ww = src.shape
@@ -506,8 +622,8 @@ def materialize(n, device):
 
 # ------------------------------------------------------------------------------------------------ module forwards
 def _require_cuda(x, what):
-    if not x.is_cuda:
-        raise RuntimeError("%s is frozen: its forward runs on the hawq_b200 CUDA kernels and needs a CUDA input "
+    if not x.is_cuda:        # NotImplementedError (a RuntimeError): this path has no CPU implementation
+        raise NotImplementedError("%s is frozen: its forward runs on the hawq_b200 CUDA kernels and needs a CUDA input "
                            "(got %s). Un-freeze the model for CPU calibration; there is no CPU fallback." % (what, x.device))
 
 
@@ -544,10 +660,11 @@ def act_forward(act, x, a_sf, w_sf, identity, id_sf, id_w_sf):
             raise NotImplementedError("QuantAct without a previous scale expects concrete integers")
         return (x, scale)
     if n.kind == "conv":
-        if n.pool is not None:                                 # stem: conv -> pool -> QuantAct(16) [-> ReLU]
+        stem3 = _conv_cache(n.mod, n.a_sf, n.src.bits if n.src.bits in (4, 8) else 8, dev)["kind"] == "stem3"
+        if n.pool is not None or stem3:                        # stem: conv -> pool -> QuantAct(16) [-> ReLU], conv -> ReLU6 -> QuantAct(16)
             st = Node("stem", n.shape, a=n, act=act)
             if act.activation_bit != 16:
-                raise NotImplementedError("pooled convolution must be followed by the 16-bit quant_act_int32")
+                raise NotImplementedError("the stem convolution must be followed by the 16-bit quant_act_int32")
             return (IntActivation(st, dev), scale)
         return (IntActivation(_conv_case0(n, act, dev), dev), scale)
     if n.kind in ("residual", "stem"):                         # fuse this activation into the producer's epilogue
@@ -560,22 +677,25 @@ def act_forward(act, x, a_sf, w_sf, identity, id_sf, id_w_sf):
         nb, c, hh, ww = src.shape
         if act.activation_bit != 8 or act.quant_mode != "symmetric":
             raise NotImplementedError("the pooled tail is 8-bit symmetric in HAWQ ResNets")
-        out = torch.empty(nb * c, dtype=torch.int8, device=dev)
-        ops.avgpool_requant(src.data, nb, hh * ww, c, src.bits, (m[0], e[0]), (lo, hi), out)
-        return (IntActivation(Node("int", (nb, c, 1, 1), data=out, bits=8, signed=True), dev), scale)
+        out = _new_int(dev, (nb, c, 1, 1), 8, True)
+        ops.avgpool_requant(src.data, nb, hh * ww, src.cs, src.bits, (m[0], e[0]), (lo, hi), out.data)
+        return (IntActivation(out, dev), scale)
     if n.kind == "int":                                        # stand-alone requant of the residual stream
         if n.bits not in (16, 32):
             raise NotImplementedError("stand-alone requantisation expects the 16/32-bit residual stream")
         ws = w_sf if w_sf is not None else _ones()
         m, e = _dyadic(act, a_sf, ws, "case0")
-        c = n.shape[1]
         per_ch = len(m) > 1
-        chan = ops.make_chan([0] * len(m), m, e).to(dev)
-        rows = int(np.prod(n.shape)) // c
+        ck = ("chan", _key(a_sf), _key(ws), n.cs, str(dev))    # cached with the (m, e) pairs: no host copy inside graph capture
+        chan = act._hawq_cache["me"].get(ck)
+        if chan is None:
+            m, e = _pad_me(m, e, n.cs)
+            chan = act._hawq_cache["me"][ck] = ops.make_chan([0] * len(m), m, e).to(dev)
+        rows = int(np.prod(n.shape)) // n.shape[1]
         lo, hi = _act_clamp(act)
-        out = _alloc(dev, n.shape, _store_bits(act))
-        ops.requant(n.data, rows, c, n.bits, chan, 1 if per_ch else 0, False, _store_bits(act), (lo, hi), out)
-        return (IntActivation(Node("int", n.shape, data=out, bits=_store_bits(act), signed=_store_signed(act)), dev), scale)
+        out = _new_int(dev, n.shape, _store_bits(act), _store_signed(act))
+        ops.requant(n.data, rows, n.cs, n.bits, chan, 1 if per_ch else 0, False, _store_bits(act), (lo, hi), out.data)
+        return (IntActivation(out, dev), scale)
     raise NotImplementedError("QuantAct on a pending %s" % n.kind)
 
 
@@ -587,11 +707,18 @@ def conv_forward(mod, x, a_sf):
     if a_sf is None:
         raise ValueError("pre_act_scaling_factor is required")
     src = materialize(x.node, x.device)
+    from .modules import QuantConv2d
+    if type(mod) is QuantConv2d and tuple(mod.conv.kernel_size) == (1, 1) and tuple(src.shape[2:]) == (1, 1):
+        # a 1x1 QuantConv2d on [N,C,1,1] with no QuantAct behind it (MobileNetV2's `output`): the classifier, fp32
+        # float(acc + bias) * (w_sf_c * a_sf) as the reference's (out * bias_sf, w_sf) (quant_modules.py:718,726-736)
+        ent = _linear_plan(mod, a_sf, x.device)
+        logits = _linear_logits(src, ent)
+        return (logits.view(src.shape[0], -1, 1, 1), ent["w_sf"])
     ent = _conv_cache(mod, a_sf, 8 if src.bits not in (4, 8) else src.bits, x.device)
     nb, _, hh, ww = src.shape
     ho = (hh + 2 * ent["pad"] - ent["k"]) // ent["stride"] + 1
     wo = (ww + 2 * ent["pad"] - ent["k"]) // ent["stride"] + 1
-    n = Node("conv", (nb, ent["cout"], ho, wo), mod=mod, src=src, a_sf=a_sf)
+    n = Node("conv", (nb, ent["cout_l"], ho, wo), mod=mod, src=src, a_sf=a_sf)
     return (IntActivation(n, x.device), ent["w_sf"])
 
 
@@ -600,31 +727,42 @@ def linear_forward(mod, x, a_sf):
     if not isinstance(x, IntActivation):
         _require_cuda(x, "QuantLinear")
         raise NotImplementedError("a frozen QuantLinear expects the IntActivation produced by a frozen QuantAct")
-    n = materialize(x.node, x.device)
+    return _linear_logits(materialize(x.node, x.device), _linear_plan(mod, a_sf, x.device))
+
+
+def _linear_plan(mod, a_sf, dev):
+    return _plan(mod, a_sf, dev, (mod.weight_bit, mod.per_channel), lambda: _linear_params(mod, a_sf, dev))
+
+
+def _linear_logits(n, ent):
+    """fp32 [N, Cout] logits of the classifier plan `ent` on concrete int8 features n (hawq_linear_i8)."""
     if n.bits != 8 or not n.signed:
-        raise NotImplementedError("QuantLinear input must be signed int8")
-    dev = x.device
-    ent = _plan(mod, a_sf, dev, (mod.weight_bit, mod.per_channel), lambda: _linear_params(mod, a_sf, dev))
+        raise NotImplementedError("classifier input must be signed int8")
+    if n.cs != ent["k"]:
+        raise RuntimeError("classifier input has %d stored features, its weights %d" % (n.cs, ent["k"]))
     nb = n.shape[0]
-    out = torch.empty((nb, ent["cout"]), dtype=torch.float32, device=dev)
+    out = torch.empty((nb, ent["cout"]), dtype=torch.float32, device=n.data.device)
     ops.linear(n.data, ent["w"], ent["chan"], ent["fscale"], out, nb, ent["k"], ent["cout"], ent["cpad"])
     return out
 
 
 def _linear_params(mod, a_sf, dev):
+    """QuantLinear, or a 1x1 QuantConv2d used as the classifier (weights [Cout, K, 1, 1])."""
     w_sf, w_int, b_int, bias_sf = mod.integer_params(a_sf.to(mod.weight.device))
-    cout, k = w_int.shape
+    cout = w_int.shape[0]
+    k = w_int[0].numel()
     if k % 64 != 0:
         raise NotImplementedError("QuantLinear in_features must be a multiple of 64")
     cpad = (cout + 63) // 64 * 64
     w = torch.zeros((cpad, k), dtype=torch.int8)
-    w[:cout] = w_int.detach().to("cpu").to(torch.int8)
+    w[:cout] = w_int.detach().to("cpu").reshape(cout, k).to(torch.int8)
     bias = np.zeros(cpad, dtype=np.int64)
     if b_int is not None:
         bias[:cout] = b_int.detach().to("cpu").to(torch.int64).numpy()
     fs = torch.zeros(cpad, dtype=torch.float32)
     fs[:cout] = bias_sf.detach().to("cpu", torch.float32).reshape(-1)   # fc_scaling_factor * act scale, fp32
-    return dict(w=w.to(dev), chan=ops.make_chan(bias, [0] * cpad, [1] * cpad).to(dev), fscale=fs.to(dev), cout=cout, cpad=cpad, k=k)
+    return dict(w=w.to(dev), chan=ops.make_chan(bias, [0] * cpad, [1] * cpad).to(dev), fscale=fs.to(dev), cout=cout, cpad=cpad, k=k,
+                w_sf=w_sf.detach().to("cpu", torch.float32))
 
 
 def avgpool_forward(mod, x, sf):

@@ -56,7 +56,12 @@ enum hawq_status {
 #define HAWQ_FLAG_REQUANT_OVERFLOW 4     /* a requantised value left int32 on the fast path (ratio > 1): re-run without HAWQ_EP_* flags */
 
 /* Per-output-channel epilogue parameters (16 B, one vector load per channel).
- * bias = bias_integer (quant_modules.py:481-484), (m, e) = batch_frexp of the requant ratio of that channel. */
+ * bias = bias_integer (quant_modules.py:481-484), (m, e) = batch_frexp of the requant ratio of that channel.
+ * reserved: with relu 2 (ReLU6) in a REQUANT epilogue, hawq_dwconv3x3 or hawq_stem3x3_i8 it is the channel's output cap: the
+ * upper clamp of channel c is min(clamp_hi, reserved), so q = max(lo', min(RHE(...), min(clamp_hi, reserved))) with the ReLU-folded
+ * lo' = min(max(clamp_lo, 0), clamp_hi).  ReLU6 (q_mobilenetv2.py) caps the accumulator at C_c = round_f32(6 / a_sf / w_sf_c), and the
+ * requantisation is monotone, so reserved = RHE(C_c * m_c / 2^e_c) (hawq_rhe_requant_host; clamp_hi when C_c >= 2^31).  With relu 0
+ * or 1 it means nothing. */
 typedef struct {
   int32_t bias;
   uint32_t m;
@@ -82,7 +87,8 @@ enum hawq_epilogue_mode {
 
 typedef struct {
   int32_t mode;           /* hawq_epilogue_mode */
-  int32_t relu;           /* REQUANT: max(acc+bias,0) before requant; RESIDUAL: max(sum,0) after the add */
+  int32_t relu;           /* REQUANT: 1 = max(acc+bias,0) before requant, 2 = that and the per-channel ReLU6 cap of hawq_chan.reserved;
+                             RESIDUAL: max(sum,0) after the add */
   /* REQUANT output */
   int32_t out_bits;       /* 4 (packed u4), 8 (int8), 16 (int16), 32 (int32) */
   int32_t clamp_lo, clamp_hi;
@@ -183,6 +189,22 @@ int hawq_maxpool_requant(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_
                          int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
                          int32_t low_lo, int32_t low_hi, void* out_low, void* stream);
 
+/* ---- MobileNetV2 (reference utils/models/q_mobilenetv2.py) --------------------------------------------------- */
+/* Depthwise 3x3 convolution, pad 1, stride 1 or 2 (Q_LinearBottleneck.conv2, groups = C) + the QuantAct that consumes it (case 0,
+ * per-channel chan[C], relu 0 / 1 / 2 as in hawq_epilogue_desc).  x: NHWC [N,H,W,C], int8 (a_bits 8; 4-bit values 0..15 in byte
+ * containers too) or packed nibbles (a_bits 4); w: int8 [3][3][C] (channel-minor); C % 16 == 0.
+ * out [N,Ho,Wo,C]: int8 (out_bits 8) or packed nibbles (out_bits 4) of max(lo', min(RHE((acc + bias) * m_c / 2^e_c), hi_c)). */
+int hawq_dwconv3x3(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_t C, int32_t stride, int32_t a_bits, const void* x,
+                   const int8_t* w, const hawq_chan* chan, int32_t relu, int32_t out_bits, int32_t clamp_lo, int32_t clamp_hi,
+                   void* out, void* stream);
+/* MobileNetV2 stem (init_block: 3x3 stride 2 pad 1, Cin 3) + quant_act_int32 (case 0, relu 0 / 1 / 2 as in hawq_epilogue_desc).
+ * x int8 [N,H,W,3]; w int8 [64][3][3][4] (channel 3 zero; a model with fewer output channels pads with zero rows and m = 0);
+ * chan[64].  y [N,Ho,Wo,64]: int16 (y_bits 16, clamp inside int16) or int32 (32).  Optionally the next QuantAct's copy
+ * clamp(RHE(y * low_m / 2^low_e), low_lo, low_hi) as int8 / packed nibbles (low_bits 8 / 4, 0 = none). */
+int hawq_stem3x3_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_t* x, const int8_t* w, const hawq_chan* chan, int32_t relu,
+                    int32_t clamp_lo, int32_t clamp_hi, int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
+                    int32_t low_lo, int32_t low_hi, void* out_low, void* stream);
+
 /* QuantAveragePool2d (quant_modules.py:585-602) + quant_act_output (q_resnet.py:131): x residual stream
  * [N,HW,C] (x_bits 16/32) -> int8 [N,C] = clamp(RHE(trunc_avg(x) * m / 2^e)). */
 int hawq_avgpool_requant(hawq_handle* h, int32_t N, int32_t HW, int32_t C, int32_t x_bits, const void* x,
@@ -227,9 +249,9 @@ int hawq_permute_weights_for_i4(int8_t* host_w, int64_t rows_times_taps, int32_t
  * kernels of this build read the OHWI part; hawq_conv2d_dual requires the layout.  `out` (Cout * K bytes) is normally w_ohwi + Cout * K, i.e. the copy is appended to the OHWI
  * tensor and announced with hawq_conv_desc.w_layout = 1.  Device pointers, asynchronous on the stream. */
 int hawq_retile_weights(hawq_handle* h, const int8_t* w_ohwi, int32_t Cout, int64_t K, int8_t* out, void* stream);
-/* debug: number of launches so far by kernel family: 0 = hawq_conv2d (wgmma implicit GEMM), 4 = hawq_conv2d_dual (both
- * convolutions of a resize-unit tail in one kernel); 6 = hawq_stem_pool_i8 (fused stem); families 1-3, 5 and 7 are unused
- * in this build and stay 0;
+/* debug: number of launches so far by kernel family: 0 = hawq_conv2d (wgmma implicit GEMM), 1 = hawq_dwconv3x3, 2 =
+ * hawq_stem3x3_i8, 4 = hawq_conv2d_dual (both convolutions of a resize-unit tail in one kernel); 6 = hawq_stem_pool_i8 (fused
+ * stem); families 3, 5 and 7 are unused in this build and stay 0;
  * -1 for an unknown family.  Lets tests assert which kernel ran. */
 int64_t hawq_debug_kernel_count(int32_t family);
 /* workspace query kept for ABI completeness: this build needs no scratch beyond caller tensors */
