@@ -82,13 +82,34 @@ def conv_work(desc, ep):
     return macs, b
 
 
-def make_chan(bias, m, e, cap=None):
-    """hawq_chan[C] as an int32 [C,4] CPU tensor (m stored by bit pattern; `cap`: the ReLU6 output caps of relu 2, in reserved)."""
+def make_chan(bias, m, e, cap=None, zero_acc=None, raw=False):
+    """hawq_chan[C] as an int32 [C,4] CPU tensor (m stored by bit pattern; `cap`: the ReLU6 output caps of relu 2, in reserved;
+    `raw`: the table of a RAW_I32 or classifier launch, whose acc + bias is stored as is and m, e are unused).
+
+    A bias outside int32 is never wrapped.  The reference's 32-bit bias quantiser clamps to [-2^31, 2^31 - 1] in fp32, where
+    2^31 - 1 rounds to 2^31: a "dead" channel (all weights 0, its weight scale clamped to 1e-8 / n) with a positive folded bias gets
+    exactly 2^31.  Its accumulator is identically 0 (`zero_acc[c]`), so a requantising table gives it RHE(2^31 * m / 2^e) from the
+    bias alone, which is stored exactly: with m = 0 (a ratio below 2^-62, flushed by dyadic()) that is 0 for any bias, and bias 0 is
+    stored; otherwise (bias / 2, m, e - 1), only while e - 1 >= 31, so that every ratio promise made from the original (m, e) pairs
+    (ratio_flags) still holds.  Any other bias outside int32 raises OverflowError."""
     c = len(bias)
+    b = np.array([int(v) for v in bias], dtype=object)
+    m = np.broadcast_to(np.asarray(m, dtype=np.uint64), (c,)).astype(np.uint64)
+    e = np.broadcast_to(np.asarray(e, dtype=np.int64), (c,)).astype(np.int64)
+    for i in np.nonzero([not -2 ** 31 <= v < 2 ** 31 for v in b])[0]:
+        exact = zero_acc is not None and zero_acc[i] and not raw
+        if exact and m[i] == 0:
+            b[i] = 0
+        elif exact and e[i] >= 32 and b[i] % 2 == 0 and -2 ** 31 <= b[i] // 2 < 2 ** 31:
+            b[i] //= 2
+            e[i] -= 1
+        else:
+            raise OverflowError("bias integer %d of channel %d leaves int32 (m = %d, e = %d, accumulator %s)"
+                                % (b[i], i, m[i], e[i], "identically 0" if zero_acc is not None and zero_acc[i] else "not known to be 0"))
     a = np.zeros((c, 4), dtype=np.int32)
-    a[:, 0] = np.asarray(bias, dtype=np.int64).astype(np.int32)
-    a[:, 1] = np.asarray(m, dtype=np.uint64).astype(np.uint32).view(np.int32)
-    a[:, 2] = np.asarray(e, dtype=np.int32)
+    a[:, 0] = b.astype(np.int64)
+    a[:, 1] = m.astype(np.uint32).view(np.int32)
+    a[:, 2] = e.astype(np.int32)
     if cap is not None:
         a[:, 3] = np.asarray(cap, dtype=np.int64).astype(np.int32)
     return torch.from_numpy(a)

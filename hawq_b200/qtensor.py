@@ -317,6 +317,8 @@ def _conv_params(mod, a_sf, a_bits, device):
     bias = np.zeros(cout_s, dtype=np.int64)
     if b_int is not None:
         bias[:cout] = b_int.detach().to("cpu").to(torch.int64).numpy()
+    zero_acc = np.ones(cout_s, dtype=bool)                         # channels whose accumulator is identically 0 (ops.make_chan)
+    zero_acc[:cout] = ~w.reshape(cout, -1).any(dim=1).numpy()
     kind = "conv"
     if cin == 3 and kh == 7 and conv.stride[0] == 2 and conv.padding[0] == 3 and cout == 64:
         kind = "stem"
@@ -345,7 +347,7 @@ def _conv_params(mod, a_sf, a_bits, device):
     tiled = kind == "conv" and torch.device(device).type == "cuda"
     return dict(w=ops.upload_weights(w, device) if tiled else w.to(device), w_layout=1 if tiled else 0, w_sf=w_sf, bias=bias,
                 cout=cout_s if kind != "stem3" else 64, cin=cin_s, cout_l=cout, k=kh, stride=conv.stride[0], pad=conv.padding[0],
-                stem=kind == "stem", kind=kind, chan={})
+                stem=kind == "stem", kind=kind, chan={}, zero_acc=zero_acc)
 
 
 def _pad_me(m, e, c):
@@ -355,12 +357,13 @@ def _pad_me(m, e, c):
     return list(m) + [0] * (c - len(m)), list(e) + [1] * (c - len(e))
 
 
-def _chan_tensor(ent, tag, m, e, device, caps=None):
-    """Cached hawq_chan table of plan `ent`; `caps`: a function giving the ReLU6 caps (computed on a cache miss only)."""
+def _chan_tensor(ent, tag, m, e, device, caps=None, raw=False):
+    """Cached hawq_chan table of plan `ent`; `caps`: a function giving the ReLU6 caps (computed on a cache miss only); `raw`: a
+    RAW_I32 table (ops.make_chan)."""
     t = ent["chan"].get(tag)
     if t is None:
         m, e = _pad_me(m, e, len(ent["bias"]))
-        t = ent["chan"][tag] = ops.make_chan(ent["bias"], m, e, caps() if caps else None).to(device)
+        t = ent["chan"][tag] = ops.make_chan(ent["bias"], m, e, caps() if caps else None, ent["zero_acc"], raw).to(device)
     return t
 
 
@@ -500,7 +503,7 @@ def _conv_case0(n, act, device):
 
 def _conv_raw(n, ent, device):
     """identity-branch conv: int32 accumulator + bias."""
-    chan = _chan_tensor(ent, "raw", [0] * ent["cout"], [1] * ent["cout"], device)
+    chan = _chan_tensor(ent, "raw", [0] * ent["cout"], [1] * ent["cout"], device, raw=True)
     out = _alloc(device, _stored_shape(n.shape), 32)
     _launch_conv(n, ent, ops.epilogue(EPI_RAW_I32, flags=_ratio_flags()), chan, out=out)
     return out
@@ -761,7 +764,12 @@ def _linear_params(mod, a_sf, dev):
         bias[:cout] = b_int.detach().to("cpu").to(torch.int64).numpy()
     fs = torch.zeros(cpad, dtype=torch.float32)
     fs[:cout] = bias_sf.detach().to("cpu", torch.float32).reshape(-1)   # fc_scaling_factor * act scale, fp32
-    return dict(w=w.to(dev), chan=ops.make_chan(bias, [0] * cpad, [1] * cpad).to(dev), fscale=fs.to(dev), cout=cout, cpad=cpad, k=k,
+    # a dead row (all weights 0) may hold the bias 2^31 (ops.make_chan); its logit float(2^31) * fs is stored as float(2^30) * 2 fs,
+    # the same fp32 value
+    dead = (bias >= 2 ** 31) & ~w.any(dim=1).numpy() & (bias % 2 == 0)
+    bias[dead] //= 2
+    fs[torch.from_numpy(dead)] *= 2
+    return dict(w=w.to(dev), chan=ops.make_chan(bias, [0] * cpad, [1] * cpad, raw=True).to(dev), fscale=fs.to(dev), cout=cout, cpad=cpad, k=k,
                 w_sf=w_sf.detach().to("cpu", torch.float32))
 
 

@@ -55,11 +55,25 @@ def rhe_shift(p, e):
 
 
 def requant(acc, m, e):
-    """RHE(acc * m / 2^e); acc int64 [..., C], m/e scalars or [C]."""
+    """RHE(acc * m / 2^e); acc int64 [..., C], m/e scalars or [C].  acc may also be 2^31: the bias integer the reference's 32-bit
+    quantiser gives a channel whose weights are all 0 (its upper bound 2^31 - 1 rounds to 2^31 in fp32), which such a channel's
+    accumulator equals (conv_bias).  Such a channel's ratio can be below 2^-62 (e > 62): |acc * m| <= 2^62 then rounds to 0."""
     acc = np.asarray(acc, dtype=I64)
     m = np.asarray(m, dtype=I64)
-    assert acc.min(initial=0) >= -2 ** 31 and acc.max(initial=0) < 2 ** 31, "accumulator leaves int32"
-    return rhe_shift(acc * m, e)
+    e = np.asarray(e, dtype=I64)
+    assert acc.min(initial=0) >= -2 ** 31 and acc.max(initial=0) <= 2 ** 31, "accumulator leaves int32"
+    assert np.all(m <= 2 ** 31)
+    return np.where(e > 62, I64(0), rhe_shift(acc * m, np.minimum(e, 62)))
+
+
+def conv_bias(acc, w, b):
+    """acc + b per output channel (acc [..., C] without bias, w [C, ...] the channel's integer weights).  A channel with a weight is an
+    int32 accumulator; one whose weights are all 0 holds its bias alone, which may be 2^31 (requant)."""
+    y = acc + b
+    if y.min(initial=0) < -2 ** 31 or y.max(initial=0) >= 2 ** 31:
+        live = np.asarray(w).reshape(len(b), -1).any(axis=1)
+        assert y[..., live].min(initial=0) >= -2 ** 31 and y[..., live].max(initial=0) < 2 ** 31, "accumulator leaves int32"
+    return y
 
 
 def requant_fp64(acc, m, e):
@@ -150,7 +164,7 @@ class IntResNet:
 
     def _conv(self, name, x):
         c = self.convs[name]
-        return conv2d_nhwc(x, c["w"], c["stride"], c["pad"]) + c["b"]
+        return conv_bias(conv2d_nhwc(x, c["w"], c["stride"], c["pad"]), c["w"], c["b"])
 
     def _case0(self, name, acc, a_sf, w_sf, relu):
         """acc -> [ReLU] -> requant(per-channel) -> clamp.  ReLU commutes with the positive-scale requant."""
@@ -271,7 +285,7 @@ class IntMobileNetV2:
     def _conv(self, name, x):
         c = self.convs[name]
         f = dwconv2d_nhwc if c["groups"] > 1 else conv2d_nhwc
-        return f(x, c["w"], c["stride"], c["pad"]) + c["b"]
+        return conv_bias(f(x, c["w"], c["stride"], c["pad"]), c["w"], c["b"])
 
     def _case0(self, name, acc, a_sf, w_sf, relu6=False):
         a = self.acts[name]
