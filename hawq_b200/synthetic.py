@@ -105,9 +105,10 @@ def synthetic_float_resnet(arch, seed=0):
 
 
 def synthetic_batch(batch, seed, hw=224):
-    """Seeded N(0,1) image batch, NCHW fp32 on CPU (the calibration / parity input)."""
+    """Seeded N(0,1) image batch, NCHW fp32 on CPU (the calibration / parity input).  hw: side of a square image, or (H, W)."""
+    h, w = (hw, hw) if isinstance(hw, int) else tuple(hw)
     g = torch.Generator().manual_seed(seed)
-    return torch.randn(batch, 3, hw, hw, generator=g)
+    return torch.randn(batch, 3, h, w, generator=g)
 
 
 # ----------------------------------------------------------------------------- MobileNetV2 (pytorchcv `mobilenetv2_w1` layout)

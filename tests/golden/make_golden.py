@@ -7,6 +7,8 @@ Outputs (small, committed):
   net_<arch>_<scheme>.npz   whole-network: act ranges, per-QuantAct checksums of the activation integers,
                             per-layer checksums of weight_integer / bias_integer, logits  (batch 2)
   net_mobilenetv2_w1_<scheme>.npz   the same for MobileNetV2-1.0 (python tests/golden/make_golden.py --mobilenetv2 uniform8|uniform4)
+  size_<arch>_<scheme>_<H>x<W>.npz   the same with the parity batch drawn at H x W instead of 224 x 224 (same model, same
+                            calibration at 224): python tests/golden/make_golden.py --size [<arch> <scheme> <H>x<W>]
 Nothing here runs on the GPU box; tests only read the .npz files.
 """
 import hashlib
@@ -32,6 +34,11 @@ NET_CONFIGS = [("resnet18", "uniform8"), ("resnet18", "uniform4"), ("resnet18", 
 NET_CONFIGS += [("resnet18", s) for s in ("modelsize_0.75", "modelsize_0.5", "modelsize_0.25", "bops_0.75", "bops_0.25", "latency_0.5")]
 NET_CONFIGS += [("resnet50", s) for s in ("modelsize_0.75", "modelsize_0.5", "modelsize_0.25", "bops_0.75", "bops_0.25",
                                           "latency_0.75", "latency_0.5", "latency_0.25")]
+# input sizes other than 224 x 224 whose last feature map is still 7 x 7 (the reference's 7 x 7 average pool): 193 gives odd maps in
+# every stage (97, 49, 25, 13, 7), H != W gives unequal ones; 200 x 216 gives 25 x 27 and 13 x 14 identity inputs to resize units
+SIZE_CONFIGS = [("resnet50", "uniform4", (193, 224)), ("resnet50", "bops_0.5", (224, 193)), ("resnet50", "modelsize_0.25", (193, 193)),
+                ("resnet50", "uniform8", (200, 216)), ("resnet18", "uniform8", (193, 193)), ("resnet18", "bops_0.5", (200, 216)),
+                ("mobilenetv2_w1", "uniform4", (193, 224)), ("mobilenetv2_w1", "bops_0.5", (224, 193))]
 
 
 def sha_i32(a):
@@ -204,15 +211,22 @@ def make_kat_modules(ns):
     np.savez_compressed(os.path.join(HERE, "kat_modules.npz"), **out)
 
 
-def make_net(ns, arch, scheme):
+def parity_input(hw):
+    """(parity batch, meta["input"], file-name suffix): 224 x 224 when hw is None, else H x W = hw"""
+    if hw is None:
+        return synthetic_batch(PARITY_BATCH, PARITY_SEED), [PARITY_BATCH, PARITY_SEED], ""
+    return synthetic_batch(PARITY_BATCH, PARITY_SEED, hw), [PARITY_BATCH, PARITY_SEED, list(hw)], "_%dx%d" % hw
+
+
+def make_net(ns, arch, scheme, hw=None):
     qm = ns.quant_modules
     net = synthetic_float_resnet(arch, 0)
     calib = synthetic_batch(CALIB_BATCH, CALIB_SEED)
     q = rh.build_reference_qresnet(arch, scheme, net, calib)
-    x = synthetic_batch(PARITY_BATCH, PARITY_SEED)
+    x, x_meta, suffix = parity_input(hw)
     logits, acts = rh.run_with_act_hooks(q, x)
     out = {"logits": logits.numpy()}
-    meta = {"arch": arch, "scheme": scheme, "calib": [CALIB_BATCH, CALIB_SEED], "input": [PARITY_BATCH, PARITY_SEED],
+    meta = {"arch": arch, "scheme": scheme, "calib": [CALIB_BATCH, CALIB_SEED], "input": x_meta,
             "acts": {}, "convs": {}, "torch": torch.__version__}
     for name, mod in q.named_modules():
         if type(mod) is qm.QuantAct:
@@ -230,11 +244,11 @@ def make_net(ns, arch, scheme):
             meta["fc"] = dict(w_sha=sha_i32(mod.weight_integer.numpy()), b_sha=sha_i32(mod.bias_integer.numpy()),
                               sf_sha=hashlib.sha256(mod.fc_scaling_factor.numpy().tobytes()).hexdigest())
     out["meta"] = np.array(json.dumps(meta))
-    np.savez_compressed(os.path.join(HERE, "net_%s_%s.npz" % (arch, scheme)), **out)
-    print(arch, scheme, "ok", logits[0, :3].tolist())
+    np.savez_compressed(os.path.join(HERE, "%s_%s_%s%s.npz" % ("size" if suffix else "net", arch, scheme, suffix)), **out)
+    print(arch, scheme, x_meta, "ok", logits[0, :3].tolist())
 
 
-def make_net_mobilenetv2(ns, scheme):
+def make_net_mobilenetv2(ns, scheme, hw=None):
     """MobileNetV2-1.0 (reference utils/models/q_mobilenetv2.py) on the synthetic skeleton: frozen logits, every QuantAct's
     integers, integer weights / biases of every convolution (depthwise ones included) and of the 1x1 classifier."""
     from hawq_b200.synthetic import synthetic_float_mobilenetv2
@@ -242,10 +256,10 @@ def make_net_mobilenetv2(ns, scheme):
     net = synthetic_float_mobilenetv2(0)
     calib = synthetic_batch(CALIB_BATCH, CALIB_SEED)
     q = rh.build_reference_qmobilenetv2(scheme, net, calib)
-    x = synthetic_batch(PARITY_BATCH, PARITY_SEED)
+    x, x_meta, suffix = parity_input(hw)
     logits, acts = rh.run_with_act_hooks(q, x)
     out = {"logits": logits.numpy()}
-    meta = {"arch": "mobilenetv2_w1", "scheme": scheme, "calib": [CALIB_BATCH, CALIB_SEED], "input": [PARITY_BATCH, PARITY_SEED],
+    meta = {"arch": "mobilenetv2_w1", "scheme": scheme, "calib": [CALIB_BATCH, CALIB_SEED], "input": x_meta,
             "acts": {}, "convs": {}, "torch": torch.__version__}
     for name, mod in q.named_modules():
         if type(mod) is qm.QuantAct:
@@ -262,8 +276,8 @@ def make_net_mobilenetv2(ns, scheme):
                                        w_bits=mod.weight_bit, shape=list(w.shape), groups=int(mod.conv.groups) if hasattr(mod, "conv") else 1,
                                        sf_sha=hashlib.sha256(sf.numpy().tobytes()).hexdigest())
     out["meta"] = np.array(json.dumps(meta))
-    np.savez_compressed(os.path.join(HERE, "net_mobilenetv2_w1_%s.npz" % scheme), **out)
-    print("mobilenetv2_w1", scheme, "ok", logits[0, :3].tolist())
+    np.savez_compressed(os.path.join(HERE, "%s_mobilenetv2_w1_%s%s.npz" % ("size" if suffix else "net", scheme, suffix)), **out)
+    print("mobilenetv2_w1", scheme, x_meta, "ok", logits[0, :3].tolist())
 
 
 def make_kat_multibranch(ns):
@@ -293,6 +307,13 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) == 3 and sys.argv[1] == "--mobilenetv2":  # e.g. --mobilenetv2 uniform8
         make_net_mobilenetv2(ns, sys.argv[2])
+        sys.exit(0)
+    if len(sys.argv) in (2, 5) and sys.argv[1] == "--size":   # every SIZE_CONFIGS entry, or one: --size resnet50 uniform4 193x224
+        for arch, scheme, hw in SIZE_CONFIGS if len(sys.argv) == 2 else [(sys.argv[2], sys.argv[3], tuple(map(int, sys.argv[4].split("x"))))]:
+            if arch == "mobilenetv2_w1":
+                make_net_mobilenetv2(ns, scheme, hw)
+            else:
+                make_net(ns, arch, scheme, hw)
         sys.exit(0)
     if len(sys.argv) == 4 and sys.argv[1] == "--net":         # one extra network golden, e.g. --net resnet101 uniform8
         make_net(ns, sys.argv[2], sys.argv[3])

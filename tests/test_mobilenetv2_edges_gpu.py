@@ -64,10 +64,10 @@ EVERY_ROW = [("uniform8", 128, (8,)), ("uniform4", 128, (8, 4)), ("modelsize_0.5
 CHUNK = 16          # images per oracle pass: a full IntMobileNetV2 trace is about 1 GB per 16 images
 
 
-def check_every_row(q, net, batch, containers, monkeypatch):
-    """Compiled logits of synthetic_batch(batch, 11) against IntMobileNetV2 on every row, and every QuantAct of every image of a checked
-    eager pass, per 4-bit container; the oracle runs CHUNK images at a time."""
-    x = synthetic_batch(batch, 11)
+def check_every_row(q, net, batch, containers, monkeypatch, hw=224):
+    """Compiled logits of synthetic_batch(batch, 11, hw) against IntMobileNetV2 on every row, and every QuantAct of every image of a
+    checked eager pass, per 4-bit container; the oracle runs CHUNK images at a time."""
+    x = synthetic_batch(batch, 11, hw)
     q_in = int_input(x, net.acts["quant_input"]["scale"])
     runs = []
     for a4 in containers:

@@ -166,14 +166,14 @@ BENCH_CONFIGS = [("resnet18", "uniform8", 8, 8), ("resnet18", "uniform4", 128, 8
 
 
 @pytest.mark.parametrize("arch,scheme,batch,a4_container", BENCH_CONFIGS)
-def test_benchmarked_configuration_matches_oracle_on_every_row(arch, scheme, batch, a4_container, monkeypatch):
+def test_benchmarked_configuration_matches_oracle_on_every_row(arch, scheme, batch, a4_container, monkeypatch, hw=224):
     """The configuration bench.py times (CUDA graph, fused kernels, uint16 stream) at the benchmarked batch size against the
     oracle (the reference's fake-quant forward restated on the CPU, oracle/fakequant.py): ALL rows of the logits bit-equal, and the
     integers of the residual stream at the end of stage 1 and of the last stage (eager pass with the same kernels) equal too.
-    Many row tiles per channel block and full-size pipelines are only reached at this size."""
+    Many row tiles per channel block and full-size pipelines are only reached at this size.  hw: the input size (synthetic_batch)."""
     monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
     _, meta = load_net_golden(arch, scheme)
-    x = synthetic_batch(batch, 11)
+    x = synthetic_batch(batch, 11, hw)
     fqm = build_fakequant(arch, scheme, meta)
     n_stage = len(fqm.units_per_stage)
     probes = ["stage1.unit%d.quant_act_int32" % fqm.units_per_stage[0], "stage%d.unit%d.quant_act_int32" % (n_stage, fqm.units_per_stage[-1])]
