@@ -96,8 +96,7 @@ extern "C" {
 int hawq_abi_version(void) { return HAWQ_ABI_VERSION; }
 const char* hawq_last_error(void) { return g_err; }
 
-int hawq_create(int device, hawq_handle** out) {
-  if (!out) return fail(HAWQ_ERR_BAD_ARG, "hawq_create: out is null");
+static int create_on(int device, hawq_handle** out) {
   CUDA_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
@@ -116,6 +115,16 @@ int hawq_create(int device, hawq_handle** out) {
     return rc;
   *out = h;
   return HAWQ_OK;
+}
+
+// handles are created per engine, from any thread: the caller's current device is left as it was
+int hawq_create(int device, hawq_handle** out) {
+  if (!out) return fail(HAWQ_ERR_BAD_ARG, "hawq_create: out is null");
+  int prev = 0;
+  CUDA_TRY(cudaGetDevice(&prev));
+  int rc = create_on(device, out);
+  cudaSetDevice(prev);
+  return rc;
 }
 
 int hawq_destroy(hawq_handle* h) {

@@ -9,15 +9,24 @@ kernel that narrows it raises a sticky device flag if a value exceeded 65535, in
 re-run with the int32 graph, so results are always exact (the reference does not clamp case-1 sums,
 ``utils/quantization_utils/quant_utils.py:456``).
 
+Several engines: each CompiledModel owns a status word (its own library handle, ``ops.using_handle``), which its graphs
+and eager runs reset, raise and copy, so engines replaying at the same time on other streams or threads neither hide nor
+borrow each other's overflow flags.  Builds (warm-up and capture) run one at a time per process: torch captures on one
+shared stream and synchronises the device when a capture begins.
+
 Multi-GPU: the path shards over images with no data-path collective (SURVEY.md §8e); ``all_gather_logits`` is the one
 NCCL exchange the benchmark config asks for.
 """
+import threading
+
 import torch
 
 from . import ops, qtensor
 from .modules import freeze_model
 from .qtensor import IntActivation, Node
 
+
+_BUILD_LOCK = threading.RLock()
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)      # transforms.Normalize of the reference's loaders (quant_train.py:357-358,
 IMAGENET_STD = (0.229, 0.224, 0.225)       # tvm_benchmark/test_resnet_accuracy_imagenet.py:82-83)
@@ -58,8 +67,15 @@ class CompiledModel:
         self.residual_bits = residual_bits
         self.input_scale = None
         self.fallbacks = 0
+        self._handle = ops.acquire_handle(self.device.index)     # this engine's status word, baked into every graph it captures
         with torch.no_grad():
             self._build(residual_bits)
+
+    def __del__(self):
+        h = self.__dict__.pop("_handle", None)
+        if h is not None:
+            self.graphs.clear()                 # the graphs that write this handle's word go first
+            ops.release_handle(self.device.index, h)
 
     # -- one eager forward on the current stream
     def _forward(self, bits, fast=True):
@@ -79,15 +95,19 @@ class CompiledModel:
         return self.model(x)
 
     def _build(self, bits, key=None):
+        with _BUILD_LOCK, ops.using_handle(self.device.index, self._handle):
+            self._build_locked(bits, key)
+
+    def _build_locked(self, bits, key):
         key = bits if key is None else key
         fast = key != "safe"                    # "safe": no ratio promises -> saturating generic kernels
         idx = self.device.index
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(s):
-            before = ops.launch_count
+            before = ops.thread_launch_count()
             out = self._forward(bits, fast)            # warm-up: builds all parameter caches
-            self.launches[key] = ops.launch_count - before
+            self.launches[key] = ops.thread_launch_count() - before
             out = self._forward(bits, fast)
             if self.gather:
                 self.gathered[key] = all_gather_logits(out, self.group)   # also initialises the NCCL communicator before capture
@@ -103,7 +123,8 @@ class CompiledModel:
             self.outs[key] = out
             return
         g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
+        # thread_local: other threads may allocate, synchronise and launch (eager runs, replays) while this capture is underway
+        with torch.cuda.graph(g, capture_error_mode="thread_local"):
             ops.reset_status(idx)
             out = self._forward(bits, fast)
             ops.copy_status(idx, self.flag)
@@ -117,9 +138,10 @@ class CompiledModel:
         if self.use_graph:
             self.graphs[key].replay()
         else:
-            ops.reset_status(self.device.index)
-            self.outs[key] = self._forward(self.bits_of[key], key != "safe")
-            ops.copy_status(self.device.index, self.flag)
+            with ops.using_handle(self.device.index, self._handle):
+                ops.reset_status(self.device.index)
+                self.outs[key] = self._forward(self.bits_of[key], key != "safe")
+                ops.copy_status(self.device.index, self.flag)
             if self.gather:
                 self.gathered[key] = all_gather_logits(self.outs[key], self.group)
                 self._gather_flags()

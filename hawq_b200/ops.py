@@ -3,8 +3,15 @@
 torch is used only as the owner of device memory and streams.  Every function launches asynchronously on
 ``torch.cuda.current_stream()`` and never synchronises, so sequences of calls can be captured in a CUDA graph.
 There is no fallback: tensors must live on a CUDA device and the in-tree library must load.
+
+Status words: every launch raises its sticky flags in the status word of a handle (hawq_create).  By default that is one handle
+per device, shared by the process.  ``using_handle`` scopes another handle to the calling thread, so that an engine
+(``CompiledModel``) owns its own word and engines that run at the same time on other streams or threads never see each
+other's flags.
 """
+import contextlib
 import ctypes as C
+import threading
 
 import numpy as np
 import torch
@@ -12,18 +19,64 @@ import torch
 from . import _lib
 from ._lib import EPI_RAW_I32, EPI_REQUANT, EPI_RESIDUAL, hawq_conv_desc, hawq_epilogue_desc
 
-_handles = {}
-launch_count = 0   # number of kernels launched through this module (bench reports it as gpu_launches)
+_handles = {}                  # device index -> the default handle
+_handles_lock = threading.Lock()
+_spare = {}                    # device index -> handles released by their owners, reused by acquire_handle
+_local = threading.local()     # per thread: the handle in scope (using_handle) and the launch counter
+
+
+def _create(device_index):
+    out = C.c_void_p()
+    _lib.check(_lib.load().hawq_create(int(device_index), C.byref(out)))
+    return out
 
 
 def handle(device_index):
+    """The handle ops on device `device_index` use on this thread: the one in scope (using_handle), else the device's default."""
+    cur = getattr(_local, "handle", None)
+    if cur is not None and cur[0] == device_index:
+        return cur[1]
     h = _handles.get(device_index)
     if h is None:
-        lib = _lib.load()
-        out = C.c_void_p()
-        _lib.check(lib.hawq_create(int(device_index), C.byref(out)))
-        h = _handles[device_index] = out
+        with _handles_lock:
+            h = _handles.get(device_index)
+            if h is None:
+                h = _handles[device_index] = _create(device_index)
     return h
+
+
+def acquire_handle(device_index):
+    """A handle of its own (its own status word) on device `device_index`, for as long as the caller holds it.  Give it back
+    with release_handle; it is then reused rather than destroyed, because hawq_destroy synchronises the device."""
+    with _handles_lock:
+        spare = _spare.get(device_index)
+        if spare:
+            return spare.pop()
+    return _create(device_index)
+
+
+def release_handle(device_index, h):
+    """Returns a handle from acquire_handle.  Its next owner (a CompiledModel) synchronises the device while it builds, before any
+    forward whose status word it reads, and resets the word at the start of each, so work still queued by the last owner cannot
+    reach it."""
+    with _handles_lock:
+        _spare.setdefault(device_index, []).append(h)
+
+
+@contextlib.contextmanager
+def using_handle(device_index, h):
+    """Every op this thread runs on device `device_index` inside the block uses handle `h` (nested scopes restore the outer one)."""
+    saved = getattr(_local, "handle", None)
+    _local.handle = (device_index, h)
+    try:
+        yield h
+    finally:
+        _local.handle = saved
+
+
+def thread_launch_count():
+    """Kernels launched through this module by the calling thread (CompiledModel reports them as gpu_launches)."""
+    return getattr(_local, "launches", 0)
 
 
 def _ctx(t):
@@ -43,14 +96,13 @@ timer = None   # set to a list to record (kernel, info, start_event, end_event) 
 def _launch(t, fn, *args, label=None, work=None):
     """Calls ABI entry point `fn`(handle, *args, stream) on the device and current stream of tensor `t` and counts the launch.
     While `timer` is set, a launch with a `label` is bracketed by CUDA events and recorded with `work()`, its (MACs, bytes)."""
-    global launch_count
     h, s = _ctx(t)
     ev0 = None
     if label is not None and timer is not None:
         ev0 = torch.cuda.Event(enable_timing=True)
         ev0.record()
     _lib.check(getattr(_lib.load(), fn)(h, *args, s))
-    launch_count += 1
+    _local.launches = thread_launch_count() + 1
     if ev0 is not None:
         info = work()
         ev1 = torch.cuda.Event(enable_timing=True)

@@ -233,10 +233,9 @@ def _frozen_scale(act):
     key = ("scale", _buf_key(act.x_min), _buf_key(act.x_max), act.activation_bit, act.quant_mode, act.__dict__.get("_override_gen", 0))
     if c.get("scale_key") != key:
         sf = act.current_scale().detach().to("cpu", torch.float32).reshape(1)
-        c["scale_key"], c["scale"] = key, sf
         act.act_scaling_factor = sf.to(act.x_min.device)
-        c["me"] = {}
-        c["gen"] = c.get("gen", 0) + 1
+        c["scale"], c["me"], c["gen"] = sf, {}, c.get("gen", 0) + 1
+        c["scale_key"] = key            # last: another thread that sees the key finds the entries it keys
     return c["scale"]
 
 
