@@ -349,18 +349,31 @@ int hawq_linear_i8(hawq_handle* h, int32_t N, int32_t K, int32_t Cout, int32_t C
   return hawq_conv2d(h, &d, &ep, x, w, chan, nullptr, nullptr, fscale, out, nullptr, stream);
 }
 
+// ResNet 7x7 / 2 stem (stem.cuh): its channel set-up and requantisation policy are conv_igemm's, over K = 147 int8 products
+static ConvParams stem_params(hawq_handle* h, int N, int H, int W, const int8_t* x, const int8_t* w, const hawq_chan* chan, int clamp_lo,
+                              int clamp_hi, void* out) {
+  ConvParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = out; p.status = h->status;
+  p.N = N; p.H = H; p.W = W; p.Cin = 3; p.Cout = 64; p.KH = 7; p.KW = 7; p.stride = 2; p.pad = 3;
+  p.Ho = (H + 6 - 7) / 2 + 1; p.Wo = (W + 6 - 7) / 2 + 1; p.K = 147;
+  p.mode = HAWQ_EPI_REQUANT; p.relu = 1; p.lo = clamp_lo; p.hi = clamp_hi;
+  set_bias_window(p, 8);
+  return p;
+}
+
 int hawq_stem_conv_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_t* x, const int8_t* w,
                       const hawq_chan* chan, int32_t clamp_lo, int32_t clamp_hi, int16_t* out, void* stream) {
   if (!h || !x || !w || !chan || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_conv_i8: null argument");
   if (N < 1 || H < 7 || W < 7) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_conv_i8: bad geometry");
   if (clamp_lo < -32768 || clamp_hi > 32767 || clamp_lo > clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_conv_i8: clamp must fit int16");
   if (N > 65535) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_conv_i8: N > 65535");
-  const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
-  const dim3 grid((Wo + STEM_TW - 1) / STEM_TW, (Ho + STEM_TH - 1) / STEM_TH, N);
+  const ConvParams p = stem_params(h, N, H, W, x, w, chan, clamp_lo, clamp_hi, out);
+  const dim3 grid((p.Wo + STEM_TW - 1) / STEM_TW, (p.Ho + STEM_TH - 1) / STEM_TH, N);
   // persistent: 4 CTAs per SM loop over the tiles and stage the weights once (round-2 A/B: 0.212 -> 0.202 ms at batch 128)
   const long long tiles = (long long)N * grid.x * grid.y;
   const int ctas = (int)(tiles < 4LL * h->sm_count ? tiles : 4LL * h->sm_count);
-  stem_conv_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(x, (const uint32_t*)w, chan, N, H, W, Ho, Wo, clamp_lo, clamp_hi, out);
+  stem_conv_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(p);
   return launch_check("stem_conv");
 }
 
@@ -435,13 +448,13 @@ int hawq_stem_pool_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int
   if (W % 16 != 0 || W > 256 || (low_bits && !dyadic_is_fast(low_m, low_e)))
     return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_pool_i8: shape / ratio outside the fused kernel (use hawq_stem_conv_i8 + hawq_maxpool_requant)");
   if (N > 65535) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_pool_i8: N > 65535");
-  const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
-  const int Po = (Ho + 2 - 3) / 2 + 1, Qo = (Wo + 2 - 3) / 2 + 1;
+  ConvParams p = stem_params(h, N, H, W, x, w256, chan, clamp_lo, clamp_hi, y);
+  p.y_bits = y_bits; p.low_bits = low_bits; p.low_m = low_m; p.low_e = low_e; p.low_lo = low_lo; p.low_hi = low_hi; p.out_low = out_low;
+  const int Po = (p.Ho + 2 - 3) / 2 + 1, Qo = (p.Wo + 2 - 3) / 2 + 1;
   const long long tiles = (long long)N * ((Po + STEMP_PH - 1) / STEMP_PH) * ((Qo + STEMP_PW - 1) / STEMP_PW);
   const int ctas = (int)(tiles < 4LL * h->sm_count ? tiles : 4LL * h->sm_count);
   ++g_kernel_count[6];
-  stem_pool_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(x, (const uint32_t*)w256, chan, N, H, W, Ho, Wo, Po, Qo, clamp_lo, clamp_hi, y_bits, y,
-                                                          low_bits, low_m, low_e, low_lo, low_hi, out_low);
+  stem_pool_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(p);
   return launch_check("stem_pool");
 }
 

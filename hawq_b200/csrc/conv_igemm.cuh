@@ -76,6 +76,26 @@ struct ChanSmem {
         Cb(reinterpret_cast<double*>(base + CB_OFF)) {}
 };
 
+// The cp.async ring of the convolution kernels (conv_igemm_kernel, conv_tail_kernel): CONV_STAGES stages of a 128-row A tile and a
+// BN-row B tile of one 64-channel k-tile, at the front of shared memory; the per-thread A copy passes and accumulator count.
+template <int BN, bool A4>
+struct ConvRing {
+  static constexpr int A_ROW = A4 ? 32 : 64;                    // bytes of one A row per k-tile (64 channels)
+  static constexpr int A_STAGE = CONV_BM * A_ROW;
+  static constexpr int B_STAGE = BN * 64;
+  static constexpr int PIPE = CONV_STAGES * (A_STAGE + B_STAGE);
+  static constexpr int A_CH = A_ROW / 16;                       // 16-byte chunks per A row: 4 or 2
+  static constexpr int A_ROWS_PER_PASS = CONV_THREADS / A_CH;   // 64 or 128
+  static constexpr int A_PASSES = CONV_BM / A_ROWS_PER_PASS;    // 2 or 1
+  static constexpr int NT = BN / 8;                             // 8-column blocks of the accumulator: 16 or 8
+  static constexpr int NACC = BN / 2;                           // accumulator registers per thread
+  static constexpr int OUT_PITCH = BN + 16;                     // low-bit staging tile, one byte per value
+};
+
+// pitch of a shared-memory tile of BN es-byte elements per row (residual operand, new stream): 8 elements of padding keep the
+// fragment-pattern reads conflict-free
+__host__ __device__ constexpr int tile_pitch(int bn, int es) { return (bn + 8) * es; }
+
 // Shared memory of one CTA.  The cp.async ring is free once the GEMM has drained, so the epilogue tiles reuse it:
 //   [ ring | uint16 residual tile ] [ channel arrays ]
 //   The uint16 residual tile has its own region: it is prefetched while the ring is in use (see gemm()).  After the GEMM the
@@ -83,21 +103,17 @@ struct ChanSmem {
 //   across the rest of the ring and the uint16 region.
 // Two CTAs per SM (what __launch_bounds__(CONV_THREADS, 2) plans for) need 2 * (TOTAL + 1 KB reserved per CTA) <= 228 KB.
 template <int BN, bool A4>
-struct ConvSmem {
-  static constexpr int A_ROW = A4 ? 32 : 64;  // bytes of one A row per k-tile (64 channels)
-  static constexpr int A_STAGE = CONV_BM * A_ROW;
-  static constexpr int B_STAGE = BN * 64;
-  static constexpr int PIPE = CONV_STAGES * (A_STAGE + B_STAGE);
-  static constexpr int OUT_PITCH = BN + 16;
-  static constexpr int OUT_STAGE = CONV_BM * OUT_PITCH;                    // low-bit output staging tile, at offset 0
-  static constexpr int RES16 = CONV_BM * (BN * 2 + 16);                    // uint16 residual tile, padded pitch
-  static constexpr int RES32 = CONV_BM * (BN * 4 + 32);                    // int32 tile, padded pitch
-  static constexpr int RES16_OFF = PIPE;
+struct ConvSmem : ConvRing<BN, A4> {
+  using R = ConvRing<BN, A4>;
+  static constexpr int OUT_STAGE = CONV_BM * R::OUT_PITCH;                 // low-bit output staging tile, at offset 0
+  static constexpr int RES16 = CONV_BM * tile_pitch(BN, 2);                // uint16 residual tile
+  static constexpr int RES32 = CONV_BM * tile_pitch(BN, 4);                // int32 tile
+  static constexpr int RES16_OFF = R::PIPE;
   static constexpr int RES32_OFF = OUT_STAGE;
-  static constexpr int MAIN = PIPE + RES16 > RES32_OFF + RES32 ? PIPE + RES16 : RES32_OFF + RES32;
+  static constexpr int MAIN = R::PIPE + RES16 > RES32_OFF + RES32 ? R::PIPE + RES16 : RES32_OFF + RES32;
   static constexpr int CHAN_OFF = MAIN;
   static constexpr int TOTAL = CHAN_OFF + ChanSmem<BN>::BYTES;
-  static_assert(OUT_STAGE <= PIPE, "the low-bit staging tile must fit in the freed ring");
+  static_assert(OUT_STAGE <= R::PIPE, "the low-bit staging tile must fit in the freed ring");
   static_assert(2 * (TOTAL + 1024) <= 228 * 1024, "two CTAs per SM must fit in shared memory");
 };
 
@@ -106,6 +122,47 @@ template <int ROW_BYTES>
 __device__ __forceinline__ int swz(int row, int ch) {
   if constexpr (ROW_BYTES == 64) return row * 64 + ((ch ^ ((row >> 1) & 3)) << 4);
   else return row * 32 + ((ch ^ ((row >> 2) & 1)) << 4);
+}
+
+// acc += one 64-channel k-tile of the ring stage at a_base / b_base (shared-memory addresses): two k32 wgmma steps of the thread's
+// warpgroup, waited for.  A4: each ldmatrix word (8 packed nibbles) is expanded with AND / SHIFT+AND into the two int8x4 words of
+// the register A fragment.
+template <int BN, bool A4>
+__device__ __forceinline__ void mma_ktile(int32_t (&acc)[BN / 2], uint32_t a_base, uint32_t b_base) {
+  constexpr int A_ROW = ConvRing<BN, A4>::A_ROW;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) {
+    const uint64_t bdesc = wgmma_desc_sw64(b_base + ks * 32);
+    if constexpr (!A4) {
+      wgmma_fence();
+      wgmma_ss<BN>(acc, wgmma_desc_sw64(a_base + (warp >> 2) * 64 * A_ROW + ks * 32), bdesc);
+    } else {
+      uint32_t r0, r1;
+      const int row = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+      ldmatrix_x2(r0, r1, a_base + swz<32>(row, ks));
+      const uint32_t af[4] = {r0 & 0x0F0F0F0Fu, r1 & 0x0F0F0F0Fu, (r0 >> 4) & 0x0F0F0F0Fu, (r1 >> 4) & 0x0F0F0F0Fu};
+      wgmma_fence();
+      wgmma_rs<BN>(acc, af, bdesc);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+  fence_operands(acc);
+}
+
+// cp.asyncs rows m0 ... m0 + CONV_BM - 1, columns n0 ... n0 + BN - 1 of the residual operand p.res (es-byte elements, Cout per row)
+// into the shared-memory tile s of pitch tile_pitch(BN, es): coalesced 16-byte copies, zero-filled past M; no commit
+template <int BN>
+__device__ __forceinline__ void load_res_tile(uint8_t* s, const ConvParams& p, int es, int m0, int n0) {
+  const int cpr = BN * es / 16;   // 16-byte chunks per row
+  const uint8_t* g = reinterpret_cast<const uint8_t*>(p.res);
+  for (int id = threadIdx.x; id < CONV_BM * cpr; id += CONV_THREADS) {
+    const int row = id / cpr, j = id - row * cpr;
+    const bool v = m0 + row < p.M;
+    const uint8_t* src = v ? g + ((size_t)(m0 + row) * p.Cout + n0) * es + j * 16 : g;
+    cp_async_16(smem_u32(s + row * tile_pitch(BN, es) + j * 16), src, v ? 16 : 0);
+  }
 }
 
 // Epilogue family of an instantiation (FAM): REQUANT to 4/8/16/32 bits, RESIDUAL, STORE (RAW_I32 and
@@ -278,13 +335,9 @@ template <int BN, bool A4, int FAM>
 __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvParams p) {
   using S = ConvSmem<BN, A4>;
   constexpr int BM = CONV_BM, STAGES = CONV_STAGES;
-  constexpr int A_ROW = S::A_ROW;
-  constexpr int A_CH = A_ROW / 16;                    // 16-byte chunks per A row: 4 or 2
-  constexpr int A_ROWS_PER_PASS = CONV_THREADS / A_CH;  // 64 or 128
-  constexpr int A_PASSES = BM / A_ROWS_PER_PASS;        // 2 or 1
+  constexpr int A_ROW = S::A_ROW, A_CH = S::A_CH, A_ROWS_PER_PASS = S::A_ROWS_PER_PASS, A_PASSES = S::A_PASSES;
+  constexpr int NT = S::NT, NACC = S::NACC;
   constexpr int B_PASSES = BN / 64;
-  constexpr int NT = BN / 8;    // 8-column blocks of the accumulator: 16 or 8
-  constexpr int NACC = BN / 2;  // accumulator registers per thread
 
   extern __shared__ __align__(1024) uint8_t smem[];   // 512-B aligned tiles: the wgmma descriptors address them swizzled
   uint8_t* sA = smem;
@@ -297,9 +350,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   const double* sCb = cs.Cb;
 
   const int tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5;
-  const int wg = warp >> 2;     // warpgroup: output rows 64 * wg ... 64 * wg + 63
-  const int g = lane >> 2, t = lane & 3;
+  const AccFrag fr(tid);   // this thread's place in the accumulator layout
   // 1-D grid, row tile major: the Cout / BN CTAs that read the same 128 activation rows are launched back to back, so all but
   // the first find those rows in L2
   const int nblk = p.Cout / BN;
@@ -311,23 +362,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
 
   int32_t acc[NACC];
 
-  // RESIDUAL operand tile in shared memory; padded pitch keeps the fragment-pattern reads conflict-free
+  // RESIDUAL operand tile in shared memory
   const int res_es = (FAM == FAM_RESIDUAL) ? ((p.res_kind == 1 || p.res_bits == 32) ? 4 : 2) : 0;
-  const int res_pitch = BN * res_es + 8 * res_es;
+  const int res_pitch = tile_pitch(BN, res_es);
   uint8_t* sRes = smem + (res_es == 2 ? S::RES16_OFF : S::RES32_OFF);
 
-  // cp.async this CTA's tile of the residual operand into sRes (coalesced 16 B, zero-fill past M); no commit
   auto load_res = [&]() {
-    if constexpr (FAM == FAM_RESIDUAL) {
-      const int cpr = BN * res_es / 16;   // 16-byte chunks per row
-      const uint8_t* gres = reinterpret_cast<const uint8_t*>(p.res);
-      for (int id = tid; id < BM * cpr; id += CONV_THREADS) {
-        const int row = id / cpr, j = id - row * cpr;
-        const bool v = m0 + row < p.M;
-        const uint8_t* src = v ? gres + ((size_t)(m0 + row) * p.Cout + n0) * res_es + j * 16 : gres;
-        cp_async_16(smem_u32(sRes + row * res_pitch + j * 16), src, v ? 16 : 0);
-      }
-    }
+    if constexpr (FAM == FAM_RESIDUAL) load_res_tile<BN>(sRes, p, res_es, m0, n0);
   };
   // the uint16 residual operand has its own region: it is fetched while the GEMM runs (the int32 operand overlaps the ring)
   const bool prefetch_res = res_es == 2;
@@ -402,26 +443,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       cp_async_commit();
 
       const int stage = kt % STAGES;
-      const uint32_t a_base = smem_u32(sA + stage * S::A_STAGE);
-      const uint32_t b_base = smem_u32(sB + stage * S::B_STAGE);
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks) {   // two k32 steps per 64-channel k-tile
-        const uint64_t bdesc = wgmma_desc_sw64(b_base + ks * 32);
-        if constexpr (!A4) {
-          wgmma_fence();
-          wgmma_ss<BN>(acc, wgmma_desc_sw64(a_base + wg * 64 * A_ROW + ks * 32), bdesc);
-        } else {
-          uint32_t r0, r1;
-          const int row = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-          ldmatrix_x2(r0, r1, a_base + swz<32>(row, ks));
-          const uint32_t af[4] = {r0 & 0x0F0F0F0Fu, r1 & 0x0F0F0F0Fu, (r0 >> 4) & 0x0F0F0F0Fu, (r1 >> 4) & 0x0F0F0F0Fu};
-          wgmma_fence();
-          wgmma_rs<BN>(acc, af, bdesc);
-        }
-      }
-      wgmma_commit();
-      wgmma_wait_all();
-      fence_operands(acc);
+      mma_ktile<BN, A4>(acc, smem_u32(sA + stage * S::A_STAGE), smem_u32(sB + stage * S::B_STAGE));
     }
     cp_async_wait<0>();
     __syncthreads();   // pipeline buffers are free
@@ -439,7 +461,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   // have the same width
   const bool y_staged = res_es != 0 && p.y_bits == res_es * 8;
   const int y_es = p.y_bits / 8;
-  const int y_pitch = BN * y_es + 8 * y_es;
+  const int y_pitch = tile_pitch(BN, y_es);
   uint8_t* sY = sRes;
 
   // ------------------------------------------------------------------------------------------------ epilogue
@@ -468,7 +490,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       const int lo = p.relu ? min(max(p.lo, 0), p.hi) : p.lo;
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
-        const int col = ni * 8 + 2 * t;
+        const int col = fr.col(ni);
         const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);   // bias, m, e (capped: upper clamp)
         const int4 c1 = *reinterpret_cast<const int4*>(&sChan[col + 1]);
         const double2 M = *reinterpret_cast<const double2*>(&sM[col]);
@@ -476,9 +498,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
         const int hi0 = FAM == FAM_REQUANT_CAPPED ? c0.w : p.hi, hi1 = FAM == FAM_REQUANT_CAPPED ? c1.w : p.hi;
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
-          const int row = warp * 16 + hf * 8 + g;
-          const int q0 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2], Cb.x, c0.x), M.x, c0.y, c0.z, false), lo, hi0);
-          const int q1 = clampi(rq.term(rq.acc_bias(acc[ni * 4 + hf * 2 + 1], Cb.y, c1.x), M.y, c1.y, c1.z, false), lo, hi1);
+          const int row = fr.row(hf);
+          const int q0 = clampi(rq.term(rq.acc_bias(acc[acc_idx(ni, hf)], Cb.x, c0.x), M.x, c0.y, c0.z, false), lo, hi0);
+          const int q1 = clampi(rq.term(rq.acc_bias(acc[acc_idx(ni, hf) + 1], Cb.y, c1.x), M.y, c1.y, c1.z, false), lo, hi1);
           if constexpr (decltype(low_out)::value) {
             put_low(row, col, q0, q1);
           } else if (m0 + row < p.M) {
@@ -495,7 +517,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
       int ymax = 0;
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
-        const int col = ni * 8 + 2 * t;
+        const int col = fr.col(ni);
         const int4 c0 = *reinterpret_cast<const int4*>(&sChan[col]);   // bias, m, e
         const int4 c1 = *reinterpret_cast<const int4*>(&sChan[col + 1]);
         const double2 M = *reinterpret_cast<const double2*>(&sM[col]);
@@ -510,7 +532,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
         }
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
-          const int row = warp * 16 + hf * 8 + g;
+          const int row = fr.row(hf);
           const bool ok = m0 + row < p.M;
           const uint8_t* rptr = sRes + row * res_pitch + col * res_es;
           decltype(rq.of_i32(0)) r0, r1;
@@ -523,8 +545,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
             r0 = rq.of_i32(pr.x);
             r1 = rq.of_i32(pr.y);
           }
-          const int y0 = residual_y(rq, rq.term(r0, M1.x, m1.x, e1.x, ok), acc[ni * 4 + hf * 2 + 0], Cb.x, c0, M.x, ok, relu_floor);
-          const int y1 = residual_y(rq, rq.term(r1, M1.y, m1.y, e1.y, ok), acc[ni * 4 + hf * 2 + 1], Cb.y, c1, M.y, ok, relu_floor);
+          const int y0 = residual_y(rq, rq.term(r0, M1.x, m1.x, e1.x, ok), acc[acc_idx(ni, hf)], Cb.x, c0, M.x, ok, relu_floor);
+          const int y1 = residual_y(rq, rq.term(r1, M1.y, m1.y, e1.y, ok), acc[acc_idx(ni, hf) + 1], Cb.y, c1, M.y, ok, relu_floor);
           put_y(row, col, ok, y0, y1, ymax);
           if (p.low_bits != 0) put_low(row, col, residual_low(rq, y0, low_M, p), residual_low(rq, y1, low_M, p));
         }
@@ -536,13 +558,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_igemm_kernel(const ConvP
   if constexpr (FAM == FAM_STORE) {   // RAW_I32: sat_add(acc, bias); DEQUANT_F32: float(acc + bias) * fscale, first cout_store columns
 #pragma unroll
     for (int ni = 0; ni < NT; ++ni) {
-      const int col = ni * 8 + 2 * t;
+      const int col = fr.col(ni);
       const int b0 = sChan[col].bias, b1 = sChan[col + 1].bias;
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
-        const int m = m0 + warp * 16 + hf * 8 + g;
+        const int m = m0 + fr.row(hf);
         if (m >= p.M) continue;
-        const int32_t v0 = sat_add(acc[ni * 4 + hf * 2 + 0], b0), v1 = sat_add(acc[ni * 4 + hf * 2 + 1], b1);
+        const int32_t v0 = sat_add(acc[acc_idx(ni, hf)], b0), v1 = sat_add(acc[acc_idx(ni, hf) + 1], b1);
         if (p.mode == HAWQ_EPI_RAW_I32) {
           *reinterpret_cast<int2*>(reinterpret_cast<int32_t*>(p.out) + (size_t)m * p.Cout + n0 + col) = make_int2(v0, v1);
         } else {

@@ -30,22 +30,18 @@ constexpr int TAIL_BN = 64;
 // [ ring | resize units: int32 identity terms | uint16 tiles (two residual slots; resize units: one stream tile) | low-bit staging ]
 // [ channel arrays ].  The new uint16 stream is staged in place over the residual tile it is computed from.
 template <bool A4, bool DUAL>
-struct TailSmem {
+struct TailSmem : ConvRing<TAIL_BN, A4> {
+  using R = ConvRing<TAIL_BN, A4>;
   static constexpr int BN = TAIL_BN;
-  static constexpr int A_ROW = A4 ? 32 : 64;
-  static constexpr int A_STAGE = CONV_BM * A_ROW;
-  static constexpr int B_STAGE = BN * 64;
-  static constexpr int PIPE = CONV_STAGES * (A_STAGE + B_STAGE);
-  static constexpr int Y_PITCH = BN * 2 + 16;            // uint16 tile, padded pitch (conflict-free fragment reads)
+  static constexpr int Y_PITCH = tile_pitch(BN, 2);      // uint16 tile
   static constexpr int Y_SLOT = CONV_BM * Y_PITCH;
-  static constexpr int I_OFF = PIPE;                     // identity terms: BN / 4 int2 per thread, [pair][thread]
+  static constexpr int I_OFF = R::PIPE;                  // identity terms: BN / 4 int2 per thread, [pair][thread]
   static constexpr int Y_OFF = I_OFF + (DUAL ? BN / 4 * CONV_THREADS * 8 : 0);
   static constexpr int Y_SLOTS = DUAL ? 1 : 2;
-  static constexpr int OUT_PITCH = BN + 16;
   static constexpr int OUT_OFF = Y_OFF + Y_SLOTS * Y_SLOT;
-  static constexpr int CHAN_OFF = OUT_OFF + CONV_BM * OUT_PITCH;
+  static constexpr int CHAN_OFF = OUT_OFF + CONV_BM * R::OUT_PITCH;
   static constexpr int TOTAL = CHAN_OFF + ChanSmem<BN>::BYTES;
-  static_assert(A_STAGE % 512 == 0 && B_STAGE % 512 == 0, "wgmma tiles must stay 512-B aligned");
+  static_assert(R::A_STAGE % 512 == 0 && R::B_STAGE % 512 == 0, "wgmma tiles must stay 512-B aligned");
   static_assert(Y_OFF % 16 == 0 && Y_SLOT % 16 == 0 && OUT_OFF % 16 == 0 && CHAN_OFF % 16 == 0, "16-byte copies need aligned tiles");
   static_assert(2 * (TOTAL + 1024) <= 228 * 1024, "two CTAs per SM must fit in shared memory");
 };
@@ -61,12 +57,8 @@ template <bool A4, bool DUAL>
 __global__ void __launch_bounds__(CONV_THREADS, 2) conv_tail_kernel(const ConvParams p) {
   using S = TailSmem<A4, DUAL>;
   constexpr int BN = TAIL_BN, BM = CONV_BM, STAGES = CONV_STAGES;
-  constexpr int A_ROW = S::A_ROW;
-  constexpr int A_CH = A_ROW / 16;
-  constexpr int A_ROWS_PER_PASS = CONV_THREADS / A_CH;
-  constexpr int A_PASSES = BM / A_ROWS_PER_PASS;
-  constexpr int NT = BN / 8;
-  constexpr int NACC = BN / 2;
+  constexpr int A_ROW = S::A_ROW, A_CH = S::A_CH, A_ROWS_PER_PASS = S::A_ROWS_PER_PASS, A_PASSES = S::A_PASSES;
+  constexpr int NT = S::NT, NACC = S::NACC;
 
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
@@ -75,9 +67,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_tail_kernel(const ConvPa
   const ChanSmem<BN> cs(smem + S::CHAN_OFF);
 
   const int tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5;
-  const int wg = warp >> 2;
-  const int g = lane >> 2, t = lane & 3;
+  const AccFrag fr(tid);   // this thread's place in the accumulator layout
 
   const int nblk = p.Cout / BN;
   const int n0 = (int)(blockIdx.x % nblk) * BN;
@@ -124,7 +114,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_tail_kernel(const ConvPa
       const int8_t* wb = ident ? p.w2 : p.w;
       const int wk = (ident ? KT2 : KT) * 64;
       cp_async_16(smem_u32(sB + ld_s * S::B_STAGE) + swz<64>(b_row, b_ch), wb + (size_t)(n0 + b_row) * wk + kc * 64 + b_ch * 16, 16);
-      if (!DUAL && ld_k == 0) {   // the tile's uint16 residual operand, into slot ld_t % 2
+      // the tile's uint16 residual operand, into slot ld_t % 2.  Written out rather than through load_res_tile: with the shared
+      // loader ptxas schedules this prologue differently and the stage-3 / 4 tails ran 0.5-1 % slower (H100 80GB HBM3, 700 W).
+      if (!DUAL && ld_k == 0) {
         uint8_t* sr = smem + S::Y_OFF + (ld_t & 1) * S::Y_SLOT;
         const uint8_t* gres = reinterpret_cast<const uint8_t*>(p.res);
         constexpr int CPR = BN * 2 / 16;
@@ -154,24 +146,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_tail_kernel(const ConvPa
     const uint32_t a_base = smem_u32(sA + cs_s * S::A_STAGE);
     const uint32_t b_base = smem_u32(sB + cs_s * S::B_STAGE);
     if (++cs_s == STAGES) cs_s = 0;
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
-      const uint64_t bdesc = wgmma_desc_sw64(b_base + ks * 32);
-      if constexpr (!A4) {
-        wgmma_fence();
-        wgmma_ss<BN>(acc, wgmma_desc_sw64(a_base + wg * 64 * A_ROW + ks * 32), bdesc);
-      } else {
-        uint32_t r0, r1;
-        const int row = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-        ldmatrix_x2(r0, r1, a_base + swz<32>(row, ks));
-        const uint32_t af[4] = {r0 & 0x0F0F0F0Fu, r1 & 0x0F0F0F0Fu, (r0 >> 4) & 0x0F0F0F0Fu, (r1 >> 4) & 0x0F0F0F0Fu};
-        wgmma_fence();
-        wgmma_rs<BN>(acc, af, bdesc);
-      }
-    }
-    wgmma_commit();
-    wgmma_wait_all();
-    fence_operands(acc);
+    mma_ktile<BN, A4>(acc, a_base, b_base);
   };
 
   for (int s = 0; s < D; ++s) issue();
@@ -190,15 +165,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_tail_kernel(const ConvPa
         for (int kt = 0; kt < KT2; ++kt) consume();
 #pragma unroll
         for (int ni = 0; ni < NT; ++ni) {
-          const int col = ni * 8 + 2 * t;
+          const int col = fr.col(ni);
           const int4 r0 = *reinterpret_cast<const int4*>(&cs.rc[col]);   // bias, m, e of the identity convolution
           const int4 r1 = *reinterpret_cast<const int4*>(&cs.rc[col + 1]);
           const double2 M1 = *reinterpret_cast<const double2*>(&cs.M1[col]);
 #pragma unroll
           for (int hf = 0; hf < 2; ++hf) {
-            const int row = warp * 16 + hf * 8 + g;
+            const int row = fr.row(hf);
             const bool ok = m0 + row < p.M;
-            const int i0 = ni * 4 + hf * 2;
+            const int i0 = acc_idx(ni, hf);
             *reinterpret_cast<int2*>(smem + S::I_OFF + ((ni * 2 + hf) * CONV_THREADS + tid) * 8) =
                 make_int2(rq.term(rq.of_i32(sat_add(acc[i0], r0.x)), M1.x, r0.y, r0.z, ok),
                           rq.term(rq.of_i32(sat_add(acc[i0 + 1], r1.x)), M1.y, r1.y, r1.z, ok));
@@ -212,16 +187,16 @@ __global__ void __launch_bounds__(CONV_THREADS, 2) conv_tail_kernel(const ConvPa
       uint8_t* sY = smem + S::Y_OFF + (DUAL ? 0 : (j & 1) * S::Y_SLOT);
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
-        const int col = ni * 8 + 2 * t;
+        const int col = fr.col(ni);
         const int4 c0 = *reinterpret_cast<const int4*>(&cs.chan[col]);   // bias, m, e
         const int4 c1 = *reinterpret_cast<const int4*>(&cs.chan[col + 1]);
         const double2 M = *reinterpret_cast<const double2*>(&cs.M[col]);
         const double2 Cb = *reinterpret_cast<const double2*>(&cs.Cb[col]);
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
-          const int row = warp * 16 + hf * 8 + g;
+          const int row = fr.row(hf);
           const bool ok = m0 + row < p.M;
-          const int i0 = ni * 4 + hf * 2;
+          const int i0 = acc_idx(ni, hf);
           uint32_t* yp = reinterpret_cast<uint32_t*>(sY + row * S::Y_PITCH + col * 2);
           int32_t t0, t1;
           if constexpr (DUAL) {

@@ -7,8 +7,11 @@
 // (21 x 38 pixels) is staged in shared memory as one 32-bit word per pixel (3 channels + 0).  With the K order
 // (kh, kw, c4) and kw padded 7 -> 8, one k32 MMA step is exactly one kernel row: the A fragment word of output
 // pixel ox at tap kw is the patch word at column 2*ox + kw, i.e. plain LDS.32 with no im2col buffer.
+//
+// The channel set-up and the requantisation policy are conv_igemm's (load_channel_block, with_rq, RqFp64 / RqExact), so the stem
+// rounds exactly like the convolution's REQUANT epilogue.
 #pragma once
-#include "common.cuh"
+#include "conv_igemm.cuh"
 
 namespace hawq {
 
@@ -17,15 +20,15 @@ constexpr int STEM_PH = 2 * STEM_TH + 5;  // 21
 constexpr int STEM_PW = 2 * STEM_TW + 6;  // 38 (one extra column for the zero-weight 8th tap)
 constexpr int STEM_WPITCH = 60;           // words per output channel in smem (7*8 = 56, padded: conflict-free)
 
-// input patch of one 8x16 output tile (origin iy0, ix0 may lie outside the image: zero fill), one word per pixel
-__device__ __forceinline__ void stem_load_patch(const int8_t* __restrict__ x, int n, int H, int W, int iy0, int ix0, uint32_t* sPatch) {
+// input patch of one 8x16 output tile (origin iy0, ix0 may lie outside the image: zero fill), one word per pixel; read-only loads
+__device__ __forceinline__ void stem_load_patch(const uint8_t* x, int n, int H, int W, int iy0, int ix0, uint32_t* sPatch) {
   for (int i = threadIdx.x; i < STEM_PH * STEM_PW; i += 256) {
     const int py = i / STEM_PW, px = i - py * STEM_PW;
     const int iy = iy0 + py, ix = ix0 + px;
     uint32_t v = 0;
     if ((unsigned)iy < (unsigned)H && (unsigned)ix < (unsigned)W) {
-      const int8_t* s = x + ((size_t)(n * H + iy) * W + ix) * 3;
-      v = (uint32_t)(uint8_t)s[0] | ((uint32_t)(uint8_t)s[1] << 8) | ((uint32_t)(uint8_t)s[2] << 16);
+      const uint8_t* s = x + ((size_t)(n * H + iy) * W + ix) * 3;
+      v = (uint32_t)__ldg(s) | ((uint32_t)__ldg(s + 1) << 8) | ((uint32_t)__ldg(s + 2) << 16);
     }
     sPatch[i] = v;
   }
@@ -54,29 +57,37 @@ __device__ __forceinline__ void stem_tile_mma(const uint32_t* sPatch, const uint
       const uint32_t* wr = sW + (8 * j + g) * STEM_WPITCH + kh * 8;
       b[0] = wr[t];
       b[1] = wr[4 + t];
-      mma_16832<false>(acc[j], a, b);
+      mma_16832(acc[j], a, b);
     }
   }
 }
 
-// tile loop of the persistent stem variant: gridDim.x CTAs, tile = (n, tile_y, tile_x) with x fastest
-__device__ __forceinline__ void stem_conv_persistent_body(const int8_t* __restrict__ x, const uint32_t* __restrict__ w,
-                                                          const hawq_chan* __restrict__ chan, int N, int H, int W, int Ho, int Wo,
-                                                          int lo, int hi, int16_t* __restrict__ out, uint32_t* sPatch, uint32_t* sW,
-                                                          hawq_chan* sChan, double* sM) {
+// channels c, c + 1 of one convolution output: max(clamp(RHE((acc + bias) * ratio), lo, hi), 0) as an int16 pair.  The ReLU comes
+// after the clamp (a negative clamp_hi gives 0), not folded into the lower bound as in conv_igemm's REQUANT.
+template <class Rq>
+__device__ __forceinline__ uint32_t stem_requant_pair(Rq& rq, const ChanSmem<64>& cs, int c, int32_t a0, int32_t a1, int lo, int hi) {
+  const int4 c0 = *reinterpret_cast<const int4*>(&cs.chan[c]);   // bias, m, e
+  const int4 c1 = *reinterpret_cast<const int4*>(&cs.chan[c + 1]);
+  const int q0 = max(clampi(rq.term(rq.acc_bias(a0, cs.Cb[c], c0.x), cs.M[c], c0.y, c0.z, false), lo, hi), 0);
+  const int q1 = max(clampi(rq.term(rq.acc_bias(a1, cs.Cb[c + 1], c1.x), cs.M[c + 1], c1.y, c1.z, false), lo, hi), 0);
+  return (uint32_t)(q0 & 0xFFFF) | ((uint32_t)(q1 & 0xFFFF) << 16);
+}
+
+// Persistent: a grid of a few CTAs per SM loops over the 8x16 tiles (tile = (n, tile_y, tile_x) with x fastest), so the 14 KB of
+// weights and the per-channel constants are staged once per CTA instead of once per tile (12 544 times per batch of 128).
+// p: x, w (64 x 56 words), chan[64], N, H, W, Ho, Wo, lo, hi -> out (int16).
+__global__ void __launch_bounds__(256) stem_conv_kernel(const ConvParams p) {
+  __shared__ uint32_t sPatch[STEM_PH * STEM_PW];
+  __shared__ uint32_t sW[64 * STEM_WPITCH];
+  __shared__ __align__(16) uint8_t smem[ChanSmem<64>::BYTES];
+  const ChanSmem<64> cs(smem);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
-  for (int i = tid; i < 64 * 56; i += 256) sW[(i / 56) * STEM_WPITCH + (i % 56)] = w[i];
-  int slow = 0;
-  if (tid < 64) {
-    const hawq_chan c = chan[tid];
-    sChan[tid] = c;
-    sM[tid] = dyadic_to_double(c.m, c.e);
-    slow = !dyadic_is_fast(c.m, c.e);
-  }
-  const bool use_slow = __syncthreads_or(slow) != 0;
-  const int tiles_x = (Wo + STEM_TW - 1) / STEM_TW, tiles_y = (Ho + STEM_TH - 1) / STEM_TH;
-  const long long total = (long long)N * tiles_y * tiles_x;
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(p.w);
+  for (int i = tid; i < 64 * 56; i += 256) sW[(i / 56) * STEM_WPITCH + (i % 56)] = __ldg(w + i);
+  const RqPolicy pol = load_channel_block<64, false>(p, 0, cs);   // its barriers also publish sW
+  const int tiles_x = (p.Wo + STEM_TW - 1) / STEM_TW, tiles_y = (p.Ho + STEM_TH - 1) / STEM_TH;
+  const long long total = (long long)p.N * tiles_y * tiles_x;
   for (long long tile = blockIdx.x; tile < total; tile += gridDim.x) {
     const int tx = (int)(tile % tiles_x);
     const int ty = (int)((tile / tiles_x) % tiles_y);
@@ -84,50 +95,26 @@ __device__ __forceinline__ void stem_conv_persistent_body(const int8_t* __restri
     const int oy0 = ty * STEM_TH, ox0 = tx * STEM_TW;
     const int iy0 = oy0 * 2 - 3, ix0 = ox0 * 2 - 3;
     __syncthreads();                                   // the previous tile's patch has been consumed
-    stem_load_patch(x, n, H, W, iy0, ix0, sPatch);
+    stem_load_patch(p.x, n, p.H, p.W, iy0, ix0, sPatch);
     __syncthreads();
     int32_t acc[8][4];
     stem_tile_mma(sPatch, sW, acc);
-    const int oy = warp;
-    const int oyg = oy0 + oy;
-    if (oyg >= Ho) continue;                           // (the barriers at the loop top are reached by every thread: no early exit)
+    const int oyg = oy0 + warp;                        // warp w owns output row w of the tile
+    if (oyg >= p.Ho) continue;                         // (the barriers at the loop top are reached by every thread: no early exit)
+    with_rq<false>(pol, p, [&](auto rq) {
 #pragma unroll
-    for (int hf = 0; hf < 2; ++hf) {
-      const int oxg = ox0 + g + hf * 8;
-      if (oxg >= Wo) continue;
-      int16_t* o = out + ((size_t)(n * Ho + oyg) * Wo + oxg) * 64;
+      for (int hf = 0; hf < 2; ++hf) {
+        const int oxg = ox0 + g + hf * 8;
+        if (oxg >= p.Wo) continue;
+        int16_t* o = reinterpret_cast<int16_t*>(p.out) + ((size_t)(n * p.Ho + oyg) * p.Wo + oxg) * 64;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int c = 8 * j + 2 * t;
-        const hawq_chan c0 = sChan[c], c1 = sChan[c + 1];
-        const int32_t v0 = sat_add(acc[j][hf * 2 + 0], c0.bias), v1 = sat_add(acc[j][hf * 2 + 1], c1.bias);
-        int32_t q0, q1;
-        if (use_slow) {
-          q0 = rhe_requant(v0, c0.m, c0.e);
-          q1 = rhe_requant(v1, c1.m, c1.e);
-        } else {
-          q0 = rhe_requant_fast(v0, sM[c]);
-          q1 = rhe_requant_fast(v1, sM[c + 1]);
+        for (int j = 0; j < 8; ++j) {
+          const int c = 8 * j + 2 * t;
+          *reinterpret_cast<uint32_t*>(o + c) = stem_requant_pair(rq, cs, c, acc[j][hf * 2], acc[j][hf * 2 + 1], p.lo, p.hi);
         }
-        q0 = max(clampi(q0, lo, hi), 0);
-        q1 = max(clampi(q1, lo, hi), 0);
-        *reinterpret_cast<uint32_t*>(o + c) = (uint32_t)(q0 & 0xFFFF) | ((uint32_t)(q1 & 0xFFFF) << 16);
       }
-    }
+    });
   }
-}
-
-// Persistent: a grid of a few CTAs per SM loops over the 8x16 tiles, so the 14 KB of weights and the per-channel constants are
-// staged once per CTA instead of once per tile (12 544 times per batch of 128).
-__global__ void __launch_bounds__(256) stem_conv_kernel(const int8_t* __restrict__ x, const uint32_t* __restrict__ w,
-                                                        const hawq_chan* __restrict__ chan, int N, int H, int W,
-                                                        int Ho, int Wo, int lo, int hi, int16_t* __restrict__ out) {
-  __shared__ uint32_t sPatch[STEM_PH * STEM_PW];
-  __shared__ uint32_t sW[64 * STEM_WPITCH];
-  __shared__ hawq_chan sChan[64];
-  __shared__ double sM[64];
-
-  stem_conv_persistent_body(x, w, chan, N, H, W, Ho, Wo, lo, hi, out, sPatch, sW, sChan, sM);
 }
 
 // one pooled pixel x 8 channels (max of non-negative int16 values): residual stream y (uint16 / int32, 0 = none) and the
@@ -203,28 +190,22 @@ __global__ void __launch_bounds__(256) maxpool_requant_kernel(const int16_t* __r
 // pixels, whose 3x3 windows cover the 7 x 15 convolution outputs starting at (2 * py0 - 1, 2 * px0 - 1): one 8x16 tile of the
 // convolution above.  Positions outside the convolution output hold 0, neutral for the max of non-negative values.
 constexpr int STEMP_PH = 3, STEMP_PW = 7;
-__global__ void __launch_bounds__(256) stem_pool_kernel(const int8_t* __restrict__ x, const uint32_t* __restrict__ w256,
-                                                        const hawq_chan* __restrict__ chan, int N, int H, int W, int Ho, int Wo,
-                                                        int Po, int Qo, int lo, int hi, int y_bits, void* __restrict__ y, int low_bits,
-                                                        uint32_t low_m, int low_e, int low_lo, int low_hi, void* __restrict__ out_low) {
+// p: x, w (64 x 64 words, kernel rows 0..6 read), chan[64], N, H, W, Ho, Wo (convolution output), lo, hi, y_bits -> out,
+// low_bits / low_m / low_e / low_lo / low_hi -> out_low.
+__global__ void __launch_bounds__(256) stem_pool_kernel(const ConvParams p) {
   __shared__ uint32_t sPatch[STEM_PH * STEM_PW];
   __shared__ uint32_t sW[64 * STEM_WPITCH];
-  __shared__ hawq_chan sChan[64];
-  __shared__ double sM[64];
+  __shared__ __align__(16) uint8_t smem[ChanSmem<64>::BYTES];
   __shared__ __align__(16) int16_t sConv[STEM_TH][STEM_TW][64];
+  const ChanSmem<64> cs(smem);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
-  for (int i = tid; i < 64 * 56; i += 256) sW[(i / 56) * STEM_WPITCH + (i % 56)] = w256[(i / 56) * 64 + (i % 56)];   // kernel rows 0..6
-  int slow = 0;
-  if (tid < 64) {
-    const hawq_chan c = chan[tid];
-    sChan[tid] = c;
-    sM[tid] = dyadic_to_double(c.m, c.e);
-    slow = !dyadic_is_fast(c.m, c.e);
-  }
-  const bool use_slow = __syncthreads_or(slow) != 0;
+  const uint32_t* w256 = reinterpret_cast<const uint32_t*>(p.w);
+  for (int i = tid; i < 64 * 56; i += 256) sW[(i / 56) * STEM_WPITCH + (i % 56)] = __ldg(w256 + (i / 56) * 64 + (i % 56));   // kernel rows 0..6
+  const RqPolicy pol = load_channel_block<64, false>(p, 0, cs);   // its barriers also publish sW
+  const int Po = (p.Ho - 1) / 2 + 1, Qo = (p.Wo - 1) / 2 + 1;      // max-pool 3x3 / 2, pad 1
   const int tiles_x = (Qo + STEMP_PW - 1) / STEMP_PW, tiles_y = (Po + STEMP_PH - 1) / STEMP_PH;
-  const long long total = (long long)N * tiles_y * tiles_x;
+  const long long total = (long long)p.N * tiles_y * tiles_x;
   for (long long tile = blockIdx.x; tile < total; tile += gridDim.x) {
     const int tx = (int)(tile % tiles_x);
     const int ty = (int)((tile / tiles_x) % tiles_y);
@@ -232,7 +213,7 @@ __global__ void __launch_bounds__(256) stem_pool_kernel(const int8_t* __restrict
     const int py0 = ty * STEMP_PH, px0 = tx * STEMP_PW;
     const int oy0 = 2 * py0 - 1, ox0 = 2 * px0 - 1;
     __syncthreads();                                   // the previous tile's patch and convolution tile have been consumed
-    stem_load_patch(x, n, H, W, oy0 * 2 - 3, ox0 * 2 - 3, sPatch);
+    stem_load_patch(p.x, n, p.H, p.W, oy0 * 2 - 3, ox0 * 2 - 3, sPatch);
     __syncthreads();
     int32_t acc[8][4];
     stem_tile_mma(sPatch, sW, acc);
@@ -240,23 +221,15 @@ __global__ void __launch_bounds__(256) stem_pool_kernel(const int8_t* __restrict
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       const int cx = g + hf * 8, oxg = ox0 + cx;
-      const bool ok = (unsigned)oyg < (unsigned)Ho && (unsigned)oxg < (unsigned)Wo;
+      const bool ok = (unsigned)oyg < (unsigned)p.Ho && (unsigned)oxg < (unsigned)p.Wo;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int c = 8 * j + 2 * t;
-        const hawq_chan c0 = sChan[c], c1 = sChan[c + 1];
-        const int32_t v0 = sat_add(acc[j][hf * 2 + 0], c0.bias), v1 = sat_add(acc[j][hf * 2 + 1], c1.bias);
-        int32_t q0, q1;
-        if (use_slow) {
-          q0 = rhe_requant(v0, c0.m, c0.e);
-          q1 = rhe_requant(v1, c1.m, c1.e);
-        } else {
-          q0 = rhe_requant_fast(v0, sM[c]);
-          q1 = rhe_requant_fast(v1, sM[c + 1]);
-        }
-        q0 = ok ? max(clampi(q0, lo, hi), 0) : 0;
-        q1 = ok ? max(clampi(q1, lo, hi), 0) : 0;
-        *reinterpret_cast<uint32_t*>(&sConv[warp][cx][c]) = (uint32_t)(q0 & 0xFFFF) | ((uint32_t)(q1 & 0xFFFF) << 16);
+        // the policy is picked per pair: with one branch around the tile's 16 pairs ptxas interleaves them and this kernel needs
+        // 118 registers instead of 56
+        uint32_t q;
+        with_rq<false>(pol, p, [&](auto rq) { q = stem_requant_pair(rq, cs, c, acc[j][hf * 2], acc[j][hf * 2 + 1], p.lo, p.hi); });
+        *reinterpret_cast<uint32_t*>(&sConv[warp][cx][c]) = ok ? q : 0u;
       }
     }
     __syncthreads();
@@ -276,7 +249,8 @@ __global__ void __launch_bounds__(256) stem_pool_kernel(const int8_t* __restrict
           mx.z = __vmaxs2(mx.z, v.z);
           mx.w = __vmaxs2(mx.w, v.w);
         }
-      pool_store(mx, ((size_t)(n * Po + po) * Qo + qo) * 64 + cg * 8, y_bits, y, low_bits, low_m, low_e, low_lo, low_hi, out_low);
+      pool_store(mx, ((size_t)(n * Po + po) * Qo + qo) * 64 + cg * 8, p.y_bits, p.out, p.low_bits, p.low_m, p.low_e, p.low_lo, p.low_hi,
+                 p.out_low);
     }
   }
 }

@@ -8,6 +8,16 @@
 
 namespace hawq {
 
+// The accumulator layout in a CTA tile whose warpgroup w owns rows 64w ... 64w + 63: the thread's column pair (j, h) is
+// d[acc_idx(j, h)] and d[acc_idx(j, h) + 1], at row row(h) and columns col(j), col(j) + 1 of AccFrag(threadIdx.x).
+__device__ __forceinline__ constexpr int acc_idx(int j, int h) { return j * 4 + h * 2; }
+struct AccFrag {
+  int warp, g, t;   // warp of the CTA, lane / 4, lane % 4
+  __device__ explicit AccFrag(int tid) : warp(tid >> 5), g((tid & 31) >> 2), t(tid & 3) {}
+  __device__ int row(int h) const { return warp * 16 + h * 8 + g; }
+  __device__ int col(int j) const { return j * 8 + 2 * t; }
+};
+
 // shared-memory matrix descriptor, K-major, SWIZZLE_64B: rows of 64 B, 8-row atoms of 512 B (SBO); the tile base must be 512-B
 // aligned so that the hardware swizzle (address bits [4,6) ^= bits [7,9)) equals swz<64> of conv_igemm.cuh
 __device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
