@@ -1,4 +1,5 @@
-"""TEST INFRASTRUCTURE: an executable numpy model of the C ABI (include/hawq_b200.h) built on oracle/int_ref.py.
+"""TEST INFRASTRUCTURE: an executable numpy model of the C ABI (include/hawq_b200.h) built on oracle/int_ref.py: every launcher
+of the ResNet and MobileNetV2 engines, the ReLU6 caps of a REQUANT epilogue with relu 2 included.
 
 Two uses:
   * ``install_cpu_backend(monkeypatch)`` replaces ``hawq_b200.ops`` launchers with this model so the host logic
@@ -80,11 +81,29 @@ def rq(v, m, e):
     return sat32(ir.requant(v, m, e))
 
 
+def chan_caps(chan):
+    """hawq_chan.reserved: the per-channel output caps of relu 2 (ReLU6)."""
+    return chan.detach().cpu().numpy().reshape(-1, 4)[:, 3].astype(I64)
+
+
+def requant_clamp(v, m, e, relu, clamp, chan):
+    """REQUANT epilogue of acc + bias = v: clamp(RHE(v * m / 2^e)) with ReLU folded into the lower bound; relu 2 (ReLU6) also
+    caps channel c at min(clamp_hi, chan[c].reserved), below which the lower bound wins."""
+    lo, hi = clamp
+    if relu:
+        v = np.maximum(v, 0)
+    q = np.clip(rq(v, m, e), lo, hi)
+    if relu == 2:
+        q = np.maximum(min(max(lo, 0), hi), np.minimum(q, np.minimum(hi, chan_caps(chan))))
+    return q
+
+
 status = {"flags": 0}
 
 
 # ---------------------------------------------------------------------------------------- ABI model
-def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None, out_low=None):
+def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None, out_low=None, logical=None):
+    """hawq_conv2d.  `logical` only feeds the launch timer."""
     n, h, wd, cin, cout = desc.N, desc.H, desc.W, desc.Cin, desc.Cout
     xa = decode(x, desc.a_bits, desc.a_bits == 8).reshape(n, h, wd, cin)
     wa = w.detach().cpu().numpy().astype(I64).reshape(-1)[:cout * desc.kh * desc.kw * cin].reshape(cout, desc.kh, desc.kw, cin)
@@ -94,9 +113,7 @@ def conv2d(x, desc, ep, w, chan, res=None, res_chan=None, fscale=None, out=None,
     bias, m, e = chan_fields(chan)
     v = sat32(acc + bias)
     if ep.mode == EPI_REQUANT:
-        if ep.relu:
-            v = np.maximum(v, 0)
-        encode_into(out, np.clip(rq(v, m, e), ep.clamp_lo, ep.clamp_hi), ep.out_bits)
+        encode_into(out, requant_clamp(v, m, e, ep.relu, (ep.clamp_lo, ep.clamp_hi), chan), ep.out_bits)
     elif ep.mode == EPI_RESIDUAL:
         if ep.res_kind == 1:
             r = decode(res, 32, True).reshape(v.shape)
@@ -137,6 +154,15 @@ def conv2d_dual(x, desc, ep, w, chan, desc2, x2, w2, chan2, out=None, out_low=No
     conv2d(x, desc, ep1, w, chan, res=raw, res_chan=chan2, out=out, out_low=out_low)
 
 
+def dwconv3x3(x, n, hh, ww, c, stride, a_bits, w, chan, relu, out_bits, clamp, out, logical=None):
+    """hawq_dwconv3x3: depthwise 3x3 pad 1 (weights [3][3][C]) + the REQUANT epilogue."""
+    xa = decode(x, a_bits, a_bits == 8).reshape(n, hh, ww, c)
+    wa = w.detach().cpu().numpy().astype(I64).reshape(3, 3, c).transpose(2, 0, 1)[..., None]
+    bias, m, e = chan_fields(chan)
+    v = sat32(ir.dwconv2d_nhwc(xa, wa, stride, 1) + bias)
+    encode_into(out, requant_clamp(v, m, e, relu, clamp, chan), out_bits)
+
+
 def linear(x, w, chan, fscale, out, n, k, cout, cout_pad):
     d = real_ops.conv_desc(n, 1, 1, k, cout_pad, 1, 1, 1, 0, 8)
     conv2d(x, d, real_ops.epilogue(EPI_DEQUANT_F32, cout_store=cout), w, chan, fscale=fscale, out=out)
@@ -149,6 +175,18 @@ def stem_conv(x, w, chan, clamp, out, n, hh, ww):
     v = sat32(ir.conv2d_nhwc(xa, wa, 2, 3) + bias)
     q = np.maximum(np.clip(rq(v, m, e), clamp[0], clamp[1]), 0)
     encode_into(out, q, 16)
+
+
+def stem3x3(x, w, chan, relu, clamp, n, hh, ww, y_bits, y, low_bits, low_me, low_clamp, out_low, logical=None):
+    """hawq_stem3x3_i8: 3x3 stride 2 pad 1 convolution of 3 channels (weights [64][3][3][4]) + the REQUANT epilogue -> stream,
+    and the next QuantAct's copy clamp(RHE(y * low_m / 2^low_e))."""
+    xa = decode(x, 8, True).reshape(n, hh, ww, 3)
+    wa = w.detach().cpu().numpy().astype(I64).reshape(64, 3, 3, 4)[..., :3]
+    bias, m, e = chan_fields(chan)
+    q = requant_clamp(sat32(ir.conv2d_nhwc(xa, wa, 2, 1) + bias), m, e, relu, clamp, chan)
+    encode_into(y, q, y_bits)
+    if low_bits:
+        encode_into(out_low, np.clip(rq(q, I64(low_me[0]), I64(low_me[1])), low_clamp[0], low_clamp[1]), low_bits)
 
 
 def stem_pool(x, w256, chan, clamp, n, hh, ww, y_bits, y, low_bits, low_me, low_clamp, out_low):
@@ -240,8 +278,8 @@ def install_cpu_backend(monkeypatch):
     """Route hawq_b200.ops launchers to this model (CPU tensors).  Test-only."""
     from hawq_b200 import ops
     status["flags"] = 0
-    for name, fn in dict(conv2d=conv2d, conv2d_dual=conv2d_dual, linear=linear, stem_conv=stem_conv, stem_pool=stem_pool, maxpool_requant=maxpool_requant,
-                         avgpool_requant=avgpool_requant, quantize_input=quantize_input, quantize_input_u8=quantize_input_u8, requant=requant,
+    for name, fn in dict(conv2d=conv2d, conv2d_dual=conv2d_dual, dwconv3x3=dwconv3x3, linear=linear, stem_conv=stem_conv, stem3x3=stem3x3,
+                         stem_pool=stem_pool, maxpool_requant=maxpool_requant, avgpool_requant=avgpool_requant, quantize_input=quantize_input, quantize_input_u8=quantize_input_u8, requant=requant,
                          add_requant=add_requant, dequant=dequant, pack_i4=pack_i4_op, unpack_i4=unpack_i4_op).items():
         monkeypatch.setattr(ops, name, fn)
     monkeypatch.setattr(ops, "reset_status", lambda idx: status.__setitem__("flags", 0))

@@ -14,9 +14,7 @@ import torch
 import hawq_b200 as hb
 from hawq_b200 import ops, qtensor
 from hawq_b200.synthetic import synthetic_batch
-from oracle import int_ref as ir
-from tests.test_engine_paths_gpu import _eager, _int8, _model, _oracle
-from tests.test_mobilenetv2_engine_cpu import int_oracle, load
+from tests.engine_harness import _eager, _oracle, assert_rows, golden_model, int8_input, int_oracle
 from tests.util import golden_act_ranges, load_net_golden
 
 pytestmark = pytest.mark.gpu
@@ -34,8 +32,8 @@ def resnet():
     xs = [synthetic_batch(8, 100 + i) for i in CLEAN] + [synthetic_batch(8, 104) * 1000.0]
     fqm = _oracle(ARCH, SCHEME, meta, SHRINK)
     want = [fqm(x).numpy() for x in xs]
-    q = _model(ARCH, SCHEME, meta, SHRINK)
-    devs = [_int8(x, meta).to(DEV) for x in xs]
+    q = golden_model(ARCH, SCHEME, meta, SHRINK)
+    devs = [int8_input(x, meta["acts"]["quant_input"]["scale"]).to(DEV) for x in xs]
     status = [_eager(q, x, residual_bits=16, checked=True)[1] for x in devs]
     assert [s & 1 for s in status] == [0, 0, 0, 1], status
     assert not any(s & 6 for s in status), status
@@ -45,22 +43,16 @@ def resnet():
 @pytest.fixture(scope="module")
 def mnv2():
     """MobileNetV2 uniform8 on its golden ranges, two batches of 8 and their IntMobileNetV2 logits."""
-    _, meta = load("uniform8")
+    _, meta = load_net_golden("mobilenetv2_w1", "uniform8")
     ranges = golden_act_ranges(meta)
     _, _, net = int_oracle("uniform8", ranges, synthetic_batch(*meta["input"]))
     xs = [synthetic_batch(8, 300 + i) * (1.0 + 0.3 * i) for i in range(2)]
     want = [net(x.numpy()) for x in xs]
     s_in = np.float32(net.acts["quant_input"]["scale"])
-    devs = [torch.from_numpy(ir.quantize_input(x.numpy(), s_in).astype(np.int8)).to(DEV) for x in xs]
+    devs = [int8_input(x, s_in).to(DEV) for x in xs]
     q = hb.build_synthetic_qresnet("mobilenetv2_w1", "uniform8", act_ranges=ranges)
     assert all(_eager(q, x, residual_bits=16, checked=True)[1] & 7 == 0 for x in devs)
     return SimpleNamespace(q=q, xs=devs, want=want)
-
-
-def assert_rows(got, want, what):
-    got = got.cpu().numpy() if torch.is_tensor(got) else got
-    assert got.shape == want.shape and np.array_equal(got, want), \
-        "%s: rows differing from the oracle: %s" % (what, np.nonzero((got != want).any(axis=1))[0][:16].tolist())
 
 
 # ------------------------------------------------------------------------------------------------ a fixed interleave
@@ -228,7 +220,7 @@ def test_one_fresh_model_compiled_by_two_threads(resnet):
     that batch and on the overflowing one: every plan either thread uses is complete on the device, and all logits equal the
     oracle."""
     r = resnet
-    q = _model(ARCH, SCHEME, r.meta, SHRINK)
+    q = golden_model(ARCH, SCHEME, r.meta, SHRINK)
     assert not any("_hawq_cache" in mod.__dict__ for mod in q.modules())
 
     def compile_and_run(k):

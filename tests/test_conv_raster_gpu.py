@@ -5,12 +5,8 @@ hawq_conv2d on a 3x3 and a strided geometry.  Same checks as the geometries of t
 model, in guarded allocations."""
 import pytest
 
-from tests.test_kernels_gpu import test_conv1x1_requant_and_residual as check_conv1x1
-from tests.test_kernels_gpu import test_conv_dual_stationary_weights as check_conv_dual
-from tests.test_kernels_gpu import test_conv_raw_and_dequant_geoms as check_conv_store
-from tests.test_kernels_gpu import test_conv_requant as check_conv_requant
-from tests.test_kernels_gpu import test_conv_residual as check_conv_residual
-from tests.test_stem_pool_io_edges_gpu import sm_count
+from tests.kernel_harness import (check_conv1x1_requant_and_residual, check_conv_dual_stationary_weights, check_conv_raw_and_dequant_geoms,
+                                  check_conv_requant, check_conv_residual, sm_count)
 
 pytestmark = pytest.mark.gpu
 
@@ -18,14 +14,14 @@ pytestmark = pytest.mark.gpu
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", [(12, 28, 28, 128, 512)])   # 74 row tiles (last one ragged) x 4 channel blocks = 296 CTAs
 def test_conv1x1_many_waves(geom, a_bits):
-    check_conv1x1(geom, a_bits)
+    check_conv1x1_requant_and_residual(geom, a_bits)
 
 
 @pytest.mark.parametrize("flag", [1, 2])
 @pytest.mark.parametrize("a_bits", [8, 4])
 @pytest.mark.parametrize("geom", [(8, 56, 56, 64, 64, 256, 1)])   # ResNet-50 stage 1: 196 row tiles x 4 channel blocks = 784 CTAs
 def test_conv_dual_many_waves(geom, a_bits, flag):
-    check_conv_dual(geom, a_bits, flag)
+    check_conv_dual_stationary_weights(geom, a_bits, flag)
 
 
 # per-image shape (H, W, Cin, kh, kw, stride, pad), each with 7 x 7 outputs per image; Cin stays small to bound the model's share
@@ -66,4 +62,4 @@ def test_conv_residual_many_waves(shape, cout, a_bits):
 @pytest.mark.parametrize("shape", list(WAVE_SHAPES))
 def test_conv_raw_and_dequant_many_waves(shape, cout, a_bits):
     """RAW_I32, and DEQUANT_F32 with an odd cout_store"""
-    check_conv_store(many_wave_geom(shape, cout), a_bits)
+    check_conv_raw_and_dequant_geoms(many_wave_geom(shape, cout), a_bits)

@@ -9,32 +9,13 @@ import torch
 from hawq_b200 import ops
 from hawq_b200._lib import EPI_RESIDUAL, dyadic
 from tests import abi_model as am
-from tests.test_kernels_gpu import DEV, RATIO_ONE, run_both
-from tests.test_kernels_gpu import test_conv1x1_requant_and_residual as check_conv1x1
-from tests.test_kernels_gpu import test_conv_dual_stationary_weights as check_conv_dual
-from tests.test_kernels_gpu import test_conv_epilogue_boundaries as check_boundaries
-from tests.test_kernels_gpu import test_conv_residual as check_residual
-from tests.test_stem_pool_io_edges_gpu import sm_count
+from tests.kernel_harness import (DEV, RATIO_ONE, check_conv1x1_requant_and_residual, check_conv_dual_stationary_weights,
+                                  check_conv_epilogue_boundaries, check_conv_residual, images_for_three_tiles, row_tile_stride, run_both)
 
 pytestmark = pytest.mark.gpu
 
-BN = 64   # the tail kernel's channel block
-
 # ResNet-50 stages: (H = W of the output, bottleneck width, Cout, identity stride of the resize unit)
 STAGES = {1: (56, 64, 256, 1), 2: (28, 128, 512, 2), 3: (14, 256, 1024, 2), 4: (7, 512, 2048, 2)}
-
-
-def row_tile_stride(cout):
-    """row tiles between the consecutive tiles of one CTA: the grid is two CTAs per SM, a multiple of Cout / 64"""
-    return max(1, 2 * sm_count() // (cout // BN))
-
-
-def images_for_three_tiles(hw, cout):
-    """the smallest batch whose row tiles give every CTA at least three, the last one ragged"""
-    n = 1
-    while -(-n * hw * hw // 128) < 3 * row_tile_stride(cout) or n * hw * hw % 128 == 0:
-        n += 1
-    return n
 
 
 @pytest.mark.parametrize("a_bits", [8, 4])
@@ -42,7 +23,7 @@ def images_for_three_tiles(hw, cout):
 def test_tail_resnet50_shapes(stage, a_bits):
     """the bottleneck tail of each stage (flags 1 and 2, 8-bit, 4-bit and no low-bit copy), and REQUANT on the same geometry"""
     hw, mid, cout, _ = STAGES[stage]
-    check_conv1x1((images_for_three_tiles(hw, cout), hw, hw, mid, cout), a_bits)
+    check_conv1x1_requant_and_residual((images_for_three_tiles(hw * hw, cout), hw, hw, mid, cout), a_bits)
 
 
 @pytest.mark.parametrize("flag", [1, 2])
@@ -50,13 +31,13 @@ def test_tail_resnet50_shapes(stage, a_bits):
 @pytest.mark.parametrize("stage", sorted(STAGES))
 def test_resize_unit_resnet50_shapes(stage, a_bits, flag):
     hw, mid, cout, s2 = STAGES[stage]
-    check_conv_dual((images_for_three_tiles(hw, cout), hw, hw, mid, 64 if stage == 1 else cout // 2, cout, s2), a_bits, flag)
+    check_conv_dual_stationary_weights((images_for_three_tiles(hw * hw, cout), hw, hw, mid, 64 if stage == 1 else cout // 2, cout, s2), a_bits, flag)
 
 
 @pytest.mark.parametrize("a_bits", [8, 4])
 def test_tail_more_ctas_than_tiles(a_bits):
     """M = 81: one ragged row tile per channel block, most CTAs of the grid get none"""
-    check_conv1x1((1, 9, 9, 64, 256), a_bits)
+    check_conv1x1_requant_and_residual((1, 9, 9, 64, 256), a_bits)
 
 
 @pytest.mark.parametrize("flags", [0, 1, 2])
@@ -64,7 +45,7 @@ def test_tail_more_ctas_than_tiles(a_bits):
 def test_tail_mixed_policies_many_tiles(a_bits, flags):
     """channel blocks of one launch on different requantisation policies (FP64, FP64 clamped and checked, Exact), with every CTA
     walking several row tiles"""
-    check_boundaries((images_for_three_tiles(28, 512), 28, 28, 128, 512, 1, 1, 1, 0), a_bits, flags)
+    check_conv_epilogue_boundaries((images_for_three_tiles(28 * 28, 512), 28, 28, 128, 512, 1, 1, 1, 0), a_bits, flags)
 
 
 @pytest.mark.parametrize("tc", [0, 1])
@@ -74,7 +55,7 @@ def test_tail_residual_epilogues_many_tiles(stage, a_bits, tc):
     """test_conv_residual's epilogues on a tail geometry with at least three row tiles per CTA: its uint16-stream cases run on the
     tail kernel, the int32 and res_kind 1 cases on conv_igemm"""
     hw, mid, cout, _ = STAGES[stage]
-    check_residual((images_for_three_tiles(hw, cout), hw, hw, mid, cout, 1, 1, 1, 0), a_bits, tc)
+    check_conv_residual((images_for_three_tiles(hw * hw, cout), hw, hw, mid, cout, 1, 1, 1, 0), a_bits, tc)
 
 
 @pytest.mark.parametrize("a_bits", [8, 4])

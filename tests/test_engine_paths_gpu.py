@@ -6,51 +6,15 @@ import pytest
 import torch
 
 import hawq_b200 as hb
-from hawq_b200 import _lib, qtensor
+from hawq_b200 import qtensor
 from hawq_b200._lib import EP_RATIOS_LE_2P20
 from hawq_b200.synthetic import synthetic_batch
 from oracle import int_ref as ir
-from tests.util import build_fakequant, golden_act_ranges, load_net_golden
+from tests.engine_harness import _eager, _oracle, golden_model, int8_input
+from tests.kernel_harness import DEV, kernel_count
+from tests.util import load_net_golden
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-
-
-def _model(arch, scheme, meta, shrink=None):
-    """Frozen model on the golden ranges; ``shrink`` = (QuantAct name, factor) scales that activation's range."""
-    q = hb.build_synthetic_qresnet(arch, scheme, act_ranges=golden_act_ranges(meta))
-    if shrink is not None:
-        act = dict(q.named_modules())[shrink[0]]
-        act.x_min.mul_(shrink[1])
-        act.x_max.mul_(shrink[1])
-    return q
-
-
-def _oracle(arch, scheme, meta, shrink=None):
-    fqm = build_fakequant(arch, scheme, meta)
-    if shrink is not None:
-        a = fqm.acts[shrink[0]]
-        a.x_min, a.x_max = a.x_min * shrink[1], a.x_max * shrink[1]
-    return fqm
-
-
-def _int8(x, meta):
-    """float NCHW batch -> int8 NHWC network input, quantised like quant_input"""
-    return torch.from_numpy(ir.quantize_input(x.numpy(), np.float32(meta["acts"]["quant_input"]["scale"])).astype(np.int8))
-
-
-def _eager(q, x, **mode):
-    """One eager frozen forward of the int8 NHWC CUDA batch x under qtensor.engine_mode(**mode); returns (logits, status word)."""
-    n, h, w, c = x.shape
-    hb.ops.reset_status(0)
-    with torch.no_grad(), qtensor.engine_mode(**mode):
-        out = q(hb.IntActivation(qtensor.Node("int", (n, c, h, w), data=x.view(-1), bits=8, signed=True), x.device))
-    torch.cuda.synchronize()
-    return out, hb.ops.get_status(0)
-
-
-def _dual_count():
-    return _lib.load().hawq_debug_kernel_count(4)
 
 
 @pytest.mark.parametrize("arch,scheme", [("resnet18", "bops_0.25"), ("resnet50", "modelsize_0.5")])
@@ -62,11 +26,11 @@ def test_run_pipelined_is_exact_with_an_overflowing_batch(arch, scheme):
     however long that takes.  Repeated with ``post`` (argmax on the device) in a fresh engine."""
     _, meta = load_net_golden(arch, scheme)
     shrink = ("stage2.unit2.quant_act_int32", 0.75)
-    q = _model(arch, scheme, meta, shrink)
+    q = golden_model(arch, scheme, meta, shrink)
     xs = [synthetic_batch(8, 100 + i) * (1000.0 if i == 4 else 1.0) for i in range(7)]
     fqm = _oracle(arch, scheme, meta, shrink)
     want = [fqm(x).numpy() for x in xs]
-    hosts = [_int8(x, meta).pin_memory() for x in xs]
+    hosts = [int8_input(x, meta["acts"]["quant_input"]["scale"]).pin_memory() for x in xs]
     devs = [h.to(DEV) for h in hosts]
     overflow = [_eager(q, x, residual_bits=16, checked=True)[1] & 1 for x in devs]
     assert overflow == [0, 0, 0, 0, 1, 0, 0], overflow
@@ -116,8 +80,8 @@ def test_requant_overflow_replays_the_saturating_graph():
     ratios = launch_ratios(shrink)
     assert 1 < max(float(r.max()) for r in ratios) <= 2.0 ** 20
     assert hb.ops.ratio_flags(*[tuple(v.tolist() for v in ir.dyadic_vec(r)) for r in ratios]) == EP_RATIOS_LE_2P20
-    q = _model(arch, scheme, meta, shrink)
-    q_in = _int8(x, meta).to(DEV)
+    q = golden_model(arch, scheme, meta, shrink)
+    q_in = int8_input(x, meta["acts"]["quant_input"]["scale"]).to(DEV)
     _, status = _eager(q, q_in, residual_bits=16, checked=True)
     assert status & 4, status
     eng = hb.compile_model(q, q_in)
@@ -133,21 +97,22 @@ def test_resize_units_without_the_dual_kernel(arch, scheme, monkeypatch):
     plus a RESIDUAL convolution; the CUDA-graph logits equal those of the dual build, for the golden batch and a batch of 32, and no
     dual kernel is launched while this engine is compiled and run."""
     logits_g, meta = load_net_golden(arch, scheme)
-    q = _model(arch, scheme, meta)
+    q = golden_model(arch, scheme, meta)
     xg = synthetic_batch(*meta["input"])
-    batches = [_int8(xg, meta).to(DEV), _int8(torch.cat([xg, synthetic_batch(30, 77) * 1.3]), meta).to(DEV)]
+    s_in = meta["acts"]["quant_input"]["scale"]
+    batches = [int8_input(xg, s_in).to(DEV), int8_input(torch.cat([xg, synthetic_batch(30, 77) * 1.3]), s_in).to(DEV)]
     dual = []
     for x in batches:
-        before = _dual_count()
+        before = kernel_count(4)
         dual.append(hb.compile_model(q, x)(x).clone())
-        assert _dual_count() > before
+        assert kernel_count(4) > before
     monkeypatch.setattr(qtensor.config, "dual", False)
-    before = _dual_count()
+    before = kernel_count(4)
     for x, want in zip(batches, dual):
         eng = hb.compile_model(q, x)
         got = eng(x)
         assert eng.fallbacks == 0
         assert torch.equal(got, want)
     torch.cuda.synchronize()
-    assert _dual_count() == before
+    assert kernel_count(4) == before
     assert np.array_equal(dual[0].cpu().numpy(), logits_g)

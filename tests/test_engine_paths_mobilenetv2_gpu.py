@@ -8,16 +8,15 @@ import pytest
 import torch
 
 import hawq_b200 as hb
-from hawq_b200 import _lib, ops
+from hawq_b200 import ops
 from hawq_b200._lib import EP_RATIOS_LE_2P20
 from hawq_b200.synthetic import synthetic_batch
 from oracle import int_ref as ir
-from tests.test_engine_paths_gpu import _eager, _int8
-from tests.test_mobilenetv2_engine_cpu import int_oracle, load
+from tests.engine_harness import _eager, int8_input, int_oracle
+from tests.kernel_harness import DEV, kernel_count
 from tests.util import golden_act_ranges, load_net_golden
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 SCHEME = "uniform8"
 P = "features.stage3.unit2"          # a case-1 unit: 32 -> 32 channels at 28 x 28, its input as the identity
 Z = P + ".quant_act_int32"
@@ -41,7 +40,7 @@ def launch_ratios(meta, f):
 def shrunk_case(log2_ratio):
     """(meta, ranges, IntMobileNetV2, the model) with Z's range shrunk until the largest ratio of P's launch is 2^log2_ratio; asserts
     that the launch keeps the LE_2P20 promise."""
-    _, meta = load(SCHEME)
+    _, meta = load_net_golden("mobilenetv2_w1", SCHEME)
     r0 = max(float(r.max()) for r in launch_ratios(meta, 1.0)[0][:2])
     f = r0 / 2.0 ** log2_ratio
     ratios, net = launch_ratios(meta, f)
@@ -51,30 +50,20 @@ def shrunk_case(log2_ratio):
     return meta, ranges, net, hb.build_synthetic_qresnet("mobilenetv2_w1", SCHEME, act_ranges=ranges)
 
 
-def int_input(x, net):
-    return torch.from_numpy(ir.quantize_input(x.numpy(), np.float32(net.acts["quant_input"]["scale"])).astype(np.int8))
-
-
-def family_counts():
-    """launches taken by the depthwise (family 1) and 3x3-stem (family 2) kernels so far"""
-    lib = _lib.load()
-    return np.array([lib.hawq_debug_kernel_count(1), lib.hawq_debug_kernel_count(2)])
-
-
 def test_requant_overflow_replays_the_saturating_graph():
     """P's largest ratio at 2^19: main terms leave int32, the eager checked pass raises flag 4, and eng(x) takes one fallback to the
     safe graph, whose logits equal an eager forward with residual_bits=32, fast_kernels=False.  Building the safe graph runs the
     forward three times through the launchers (warm-up, second pass, capture), each with 17 depthwise and 1 stem launch."""
     _, _, net, q = shrunk_case(19)
-    x = int_input(synthetic_batch(2, 5), net).to(DEV)
+    x = int8_input(synthetic_batch(2, 5), net.acts["quant_input"]["scale"]).to(DEV)
     _, status = _eager(q, x, residual_bits=16, checked=True)
     assert status & 4, status
     eng = hb.compile_model(q, x)
-    before = family_counts()
+    before = [kernel_count(1), kernel_count(2)]
     got = eng(x).clone()
     torch.cuda.synchronize()
     assert eng.fallbacks == 1 and "safe" in eng.graphs
-    assert (family_counts() - before).tolist() == [3 * 17, 3 * 1]
+    assert [kernel_count(1) - before[0], kernel_count(2) - before[1]] == [3 * 17, 3 * 1]
     want, status = _eager(q, x, residual_bits=32, fast_kernels=False)
     assert status & 7 == 0
     assert torch.equal(got, want)
@@ -89,7 +78,7 @@ def test_run_pipelined_takes_the_saturating_fallback_for_every_batch():
     an eager forward in the safe graph's mode."""
     _, _, net, q = shrunk_case(19)
     xs = [synthetic_batch(8, 400 + i) * (1.3 if i == 3 else 1.0) for i in range(6)]
-    hosts = [int_input(x, net).pin_memory() for x in xs]
+    hosts = [int8_input(x, net.acts["quant_input"]["scale"]).pin_memory() for x in xs]
     devs = [h.to(DEV) for h in hosts]
     flags = [_eager(q, x, residual_bits=16, checked=True)[1] & 7 for x in devs]
     assert flags == [4] * len(xs), flags
@@ -107,14 +96,14 @@ def test_mobilenetv2_and_resnet50_replayed_alternately_on_one_stream():
     replayed alternately on one stream, three rounds, each equals its golden logits (MobileNetV2: exactly IntMobileNetV2, and the
     reference's fp32-summed logits closely) and raises no flag."""
     logits_r, meta_r = load_net_golden("resnet50", "uniform8")
-    xr = _int8(synthetic_batch(*meta_r["input"]), meta_r).to(DEV)
+    xr = int8_input(synthetic_batch(*meta_r["input"]), meta_r["acts"]["quant_input"]["scale"]).to(DEV)
     qr = hb.build_synthetic_qresnet("resnet50", "uniform8", act_ranges=golden_act_ranges(meta_r))
-    logits_m, meta_m = load(SCHEME)
+    logits_m, meta_m = load_net_golden("mobilenetv2_w1", SCHEME)
     xm_f = synthetic_batch(*meta_m["input"])
     _, _, net = int_oracle(SCHEME, golden_act_ranges(meta_m), xm_f)
     want_m = net(xm_f.numpy())
     assert np.allclose(want_m, logits_m, rtol=2e-6, atol=2e-7) and np.array_equal(want_m.argmax(1), logits_m.argmax(1))
-    xm = int_input(xm_f, net).to(DEV)
+    xm = int8_input(xm_f, net.acts["quant_input"]["scale"]).to(DEV)
     qm = hb.build_synthetic_qresnet("mobilenetv2_w1", SCHEME, act_ranges=golden_act_ranges(meta_m))
     em = hb.compile_model(qm, xm)
     er = hb.compile_model(qr, xr)

@@ -13,31 +13,15 @@ import hawq_b200 as hb
 from hawq_b200 import _lib, ops, qtensor
 from hawq_b200._lib import EPI_RESIDUAL, dyadic
 from hawq_b200.synthetic import synthetic_batch
-from oracle import int_ref as ir
-from tests.test_conv_tail_gpu import row_tile_stride
-from tests.test_input_sizes_cpu import SIZE_GOLDENS, check_engine_against_golden, engine_outputs, load_size_golden, oracle_for
-from tests.test_kernels_gpu import DEV, make_chan, out_buf, rand_act, run_both
-from tests.test_kernels_gpu import test_conv1x1_requant_and_residual as check_conv1x1
-from tests.test_kernels_gpu import test_conv_raw_and_dequant_geoms as check_raw_and_dequant
-from tests.test_kernels_gpu import test_conv_requant as check_requant
-from tests.test_kernels_gpu import test_conv_residual as check_residual
-from tests.test_kernels_gpu import test_stem_and_pool as check_stem_and_pool
-from tests.test_mobilenetv2_edges_gpu import IO, check_every_row, dw_rect
-from tests.test_mobilenetv2_edges_gpu import test_stem3x3_non_square as check_stem3x3
-from tests.test_network_gpu import MIXED_WIDTH_RESIZE
-from tests.test_network_gpu import test_benchmarked_configuration_matches_oracle_on_every_row as check_bench_resnet
+from tests.engine_harness import (MIXED_WIDTH_RESIZE, SIZE_GOLDENS, check_benchmarked_configuration_matches_oracle_on_every_row,
+                                  check_engine_against_golden, check_every_row, engine_outputs, golden_model, int8_input,
+                                  load_size_golden, oracle_for)
+from tests.kernel_harness import (DEV, IO, check_conv1x1_requant_and_residual, check_conv_raw_and_dequant_geoms, check_conv_requant,
+                                  check_conv_residual, check_stem3x3_non_square, check_stem_and_pool, dw_rect, images_for_three_tiles,
+                                  make_chan, out_buf, rand_act, run_both)
 from tests.util import golden_act_ranges, load_net_golden
 
 pytestmark = pytest.mark.gpu
-
-
-def images_for_three_tiles(m_img, cout):
-    """the smallest batch of m_img output pixels per image whose row tiles give every CTA of the tail kernel at least three, the last
-    one ragged (tests/test_conv_tail_gpu.py's rule for H x W maps)"""
-    n = 1
-    while -(-n * m_img // 128) < 3 * row_tile_stride(cout) or n * m_img % 128 == 0:
-        n += 1
-    return n
 
 
 # ------------------------------------------------------------------------------------------------ resize units, odd identity inputs
@@ -97,13 +81,13 @@ def test_conv_dual_odd_identity_inputs(case, a_bits, flag):
                                   (7, 25, 27, 128, 256, 3, 3, 2, 1),     # ResNet-18 stage-3 conv1 at 200 x 216
                                   (5, 49, 49, 256, 128, 1, 1, 2, 0)])    # ResNet-50 stage-2 conv1 at 193 x 193
 def test_strided_conv_requant_odd_maps(geom, a_bits, tc):
-    check_requant(geom, a_bits, tc)
+    check_conv_requant(geom, a_bits, tc)
 
 
 @pytest.mark.parametrize("a_bits", [8, 4])
 def test_resnet18_strided_identity_raw(a_bits):
     """ResNet-18's 1x1/2 identity convolution (RAW_I32) from 25 x 27"""
-    check_raw_and_dequant((7, 25, 27, 128, 256, 1, 1, 2, 0), a_bits)
+    check_conv_raw_and_dequant_geoms((7, 25, 27, 128, 256, 1, 1, 2, 0), a_bits)
 
 
 @pytest.mark.parametrize("tc", [0, 1])
@@ -114,7 +98,7 @@ def test_resnet18_strided_identity_raw(a_bits):
 def test_residual_odd_maps(geom, a_bits, tc):
     """RESIDUAL epilogues on odd maps; a batch of None gives every CTA of the tail kernel at least three row tiles"""
     n, h, w, cin, cout = geom[:5]
-    check_residual((n or images_for_three_tiles(h * w, cout),) + geom[1:], a_bits, tc)
+    check_conv_residual((n or images_for_three_tiles(h * w, cout),) + geom[1:], a_bits, tc)
 
 
 @pytest.mark.parametrize("a_bits", [8, 4])
@@ -122,7 +106,7 @@ def test_residual_odd_maps(geom, a_bits, tc):
 def test_bottleneck_tail_odd_maps(hw, a_bits):
     h, w = hw
     mid, cout = (256, 1024) if h == 13 else (128, 512)
-    check_conv1x1((images_for_three_tiles(h * w, cout), h, w, mid, cout), a_bits)
+    check_conv1x1_requant_and_residual((images_for_three_tiles(h * w, cout), h, w, mid, cout), a_bits)
 
 
 @pytest.mark.parametrize("shape", [(2, 193, 224), (1, 224, 193), (2, 200, 216), (3, 193, 193)])
@@ -133,7 +117,7 @@ def test_resnet_stem_odd_maps(shape):
 
 @pytest.mark.parametrize("hw", [(193, 193), (193, 224), (224, 193)])
 def test_mobilenet_stem_odd_maps(hw):
-    check_stem3x3(hw)
+    check_stem3x3_non_square(hw)
 
 
 # MobileNetV2's stride-2 depthwise convolutions at 193 x 224: (stored channels, input H, W)
@@ -149,14 +133,6 @@ def test_dwconv_stride2_odd_maps(geom):
 
 
 # ------------------------------------------------------------------------------------------------ networks against the size goldens
-def _model(meta):
-    return hb.build_synthetic_qresnet(meta["arch"], meta["scheme"], act_ranges=golden_act_ranges(meta))
-
-
-def int8_input(x, meta):
-    """NHWC int8 network input, quantised like the reference's quant_input"""
-    return torch.from_numpy(ir.quantize_input(x.numpy(), np.float32(meta["acts"]["quant_input"]["scale"])).astype(np.int8)).to(DEV)
-
 
 def int_activation(q_in):
     n, h, w, c = q_in.shape
@@ -178,7 +154,7 @@ def test_eager_module_api_matches_size_golden(name):
     the reference's, every residual-unit output equals the oracle's stream, ResNet logits bit-equal to the reference."""
     logits_g, meta, x = load_size_golden(name)
     _, _, net = oracle_for(meta, x)
-    q = _model(meta)
+    q = golden_model(meta["arch"], meta["scheme"], meta)
     for res_bits in (32, 16):
         qtensor.config.residual_bits = res_bits
         try:
@@ -208,10 +184,10 @@ def test_compiled_graph_matches_size_golden(name, a4_container, monkeypatch):
     arch, scheme = meta["arch"], meta["scheme"]
     _, _, net = oracle_for(meta, xg)
     want = golden_rows(meta, logits_g, net, xg)
-    q = _model(meta)
+    q = golden_model(meta["arch"], meta["scheme"], meta)
     B = 32
     x = torch.cat([xg, synthetic_batch(B - xg.shape[0], 77, tuple(xg.shape[2:])) * 1.3], dim=0)
-    q_in = int8_input(x, meta)
+    q_in = int8_input(x, meta["acts"]["quant_input"]["scale"]).to(DEV)
     eng = hb.compile_model(q, q_in)
     out1 = eng(q_in).clone()
     out2 = eng().clone()
@@ -246,7 +222,7 @@ def test_compiled_graph_uint8_pixels_with_a_tail_byte():
     graph ends on a partial word and must still equal the torch pipeline fed to the eager model."""
     from hawq_b200.engine import IMAGENET_MEAN, IMAGENET_STD
     _, meta, _ = load_size_golden("size_resnet18_uniform8_193x193.npz")
-    q = _model(meta)
+    q = golden_model(meta["arch"], meta["scheme"], meta)
     u8 = torch.randint(0, 256, (3, 193, 193, 3), generator=torch.Generator().manual_seed(5), dtype=torch.uint8)
     assert u8.numel() % 4 == 1
     x = u8.permute(0, 3, 1, 2).to(torch.float32).div(255)
@@ -263,14 +239,14 @@ def test_compiled_graph_uint8_pixels_with_a_tail_byte():
 @pytest.mark.parametrize("a4_container", [8, 4])
 def test_resnet50_benchmarked_batch_193x224(a4_container, monkeypatch):
     """every logits row and the stage-end residual streams of 128 images at 193 x 224 against the CPU oracle"""
-    check_bench_resnet("resnet50", "uniform4", 128, a4_container, monkeypatch, hw=(193, 224))
+    check_benchmarked_configuration_matches_oracle_on_every_row("resnet50", "uniform4", 128, a4_container, monkeypatch, hw=(193, 224))
 
 
 def test_mobilenetv2_benchmarked_batch_224x193(monkeypatch):
     """every logits row and every QuantAct of 128 images at 224 x 193 against the exact integer restatement"""
     _, meta, xg = load_size_golden("size_mobilenetv2_w1_uniform4_193x224.npz")
     _, _, net = oracle_for(meta, xg)
-    check_every_row(_model(meta), net, 128, (8, 4), monkeypatch, hw=(224, 193))
+    check_every_row(golden_model(meta["arch"], meta["scheme"], meta), net, 128, (8, 4), monkeypatch, hw=(224, 193))
 
 
 # ------------------------------------------------------------------------------------------------ one model, several sizes
@@ -282,14 +258,14 @@ def test_one_model_several_input_sizes():
     logits_s, meta_s, x_s = load_size_golden("size_resnet50_uniform4_193x224.npz")
     assert golden_act_ranges(meta_224) == golden_act_ranges(meta_s)
     x_224 = synthetic_batch(*meta_224["input"])
-    q = _model(meta_224)
+    q = golden_model(meta_224["arch"], meta_224["scheme"], meta_224)
     with torch.no_grad():
         for x, want in [(x_224, logits_224), (x_s, logits_s), (x_224, logits_224)]:
             assert np.array_equal(q(x.to(DEV)).cpu().numpy(), want), tuple(x.shape)
     engines = []
     for x, want in [(x_224, logits_224), (x_s, logits_s)]:
         xb = torch.cat([x, synthetic_batch(6, 78, tuple(x.shape[2:]))], dim=0)
-        q_in = int8_input(xb, meta_224)
+        q_in = int8_input(xb, meta_224["acts"]["quant_input"]["scale"]).to(DEV)
         eng = hb.compile_model(q, q_in)
         engines.append((eng, q_in, want))
     for _ in range(2):

@@ -1,59 +1,24 @@
-"""The frozen MobileNetV2 forward through the host engine (qtensor.py) with the kernels replaced by the ABI model (tests/abi_model.py
-and tests/abi_model_mobilenetv2.py): every QuantAct integer tensor against the reference-generated goldens, the logits against the
-exact integer restatement, zero padded channels, and ReLU6 caps that bind."""
-import json
-import os
-
+"""The frozen MobileNetV2 forward through the host engine (qtensor.py) with the kernels replaced by the ABI model (tests/abi_model.py):
+every QuantAct integer tensor against the reference-generated goldens, the logits against the exact integer restatement, zero padded
+channels, and ReLU6 caps that bind."""
 import numpy as np
 import pytest
-import torch
 
 import hawq_b200 as hb
 from hawq_b200 import qtensor
 from hawq_b200.synthetic import synthetic_batch, synthetic_float_mobilenetv2
-from oracle import fakequant as fq
 from oracle import int_ref as ir
 from tests import abi_model as am
-from tests import abi_model_mobilenetv2 as amm
-from tests.util import GOLDEN, golden_act_ranges, sha_i32
-
-SCHEMES = ["uniform8", "uniform4", "modelsize_0.5", "bops_0.5"]
-
-
-def load(scheme):
-    z = np.load(os.path.join(GOLDEN, "net_mobilenetv2_w1_%s.npz" % scheme), allow_pickle=False)
-    return z["logits"], json.loads(str(z["meta"]))
-
-
-def nhwc(a):
-    return a.transpose(0, 2, 3, 1) if a.ndim == 4 else a
-
-
-def run_engine(q, x):
-    """Frozen forward on the CPU ABI model; returns (logits, {QuantAct name: output IntActivation})."""
-    rec = {}
-    for name, m in q.named_modules():
-        if isinstance(m, hb.QuantAct):
-            m.register_forward_hook(lambda mod, inp, out, name=name: rec.__setitem__(name, out[0]))
-    with torch.no_grad():
-        y = q(x)
-    return y, rec
-
-
-def int_oracle(scheme, ranges, x, net=None):
-    o = fq.FakeQuantMobileNetV2(net if net is not None else synthetic_float_mobilenetv2(0), hb.get_bit_config("mobilenetv2_w1", scheme))
-    o.load_act_ranges(ranges)
-    o.freeze()
-    yf = o(x, trace=True)
-    return o, yf, ir.IntMobileNetV2(o.harvest())
+from tests.engine_harness import SCHEMES, int_oracle, nhwc, run_engine
+from tests.util import golden_act_ranges, load_net_golden, sha_i32
 
 
 @pytest.mark.parametrize("a4_container", [8, 4])
 @pytest.mark.parametrize("scheme", SCHEMES)
 def test_every_quantact_and_the_logits_match(scheme, a4_container, monkeypatch):
-    amm.install_cpu_backend(monkeypatch)
+    am.install_cpu_backend(monkeypatch)
     monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
-    logits_g, meta = load(scheme)
+    logits_g, meta = load_net_golden("mobilenetv2_w1", scheme)
     x = synthetic_batch(*meta["input"])
     q = hb.build_synthetic_qresnet("mobilenetv2_w1", scheme, act_ranges=golden_act_ranges(meta))
     y, rec = run_engine(q, x)
@@ -76,9 +41,9 @@ def test_relu6_caps_that_bind_equal_the_reference_arithmetic(monkeypatch):
     convolution's BN scale is multiplied by 16 and the activation range set to x_max = 8, so values above 6 reach ReLU6 and its cap
     binds below the clamp; the engine must still give the reference's float arithmetic's integers (FakeQuantMobileNetV2) at every
     QuantAct."""
-    amm.install_cpu_backend(monkeypatch)
+    am.install_cpu_backend(monkeypatch)
     scheme = "uniform8"
-    _, meta = load(scheme)
+    _, meta = load_net_golden("mobilenetv2_w1", scheme)
     ranges = golden_act_ranges(meta)
     narrowed = ["features.stage2.unit1.quant_act1", "features.stage2.unit2.quant_act2", "features.stage4.unit3.quant_act2",
                 "features.stage5.unit1.quant_act1"]

@@ -10,53 +10,16 @@ from hawq_b200 import ops, qtensor
 from hawq_b200._lib import EPI_REQUANT, dyadic
 from hawq_b200.synthetic import synthetic_batch
 from oracle import int_ref as ir
-from tests import abi_model as am
-from tests import abi_model_mobilenetv2 as amm
-from tests.test_kernels_gpu import out_buf, rand_act, widest_row_bytes
-from tests.test_mobilenetv2_engine_cpu import SCHEMES, int_oracle, load, nhwc, run_engine
-from tests.util import golden_act_ranges, guarded_call, sha_i32
+from tests.engine_harness import SCHEMES, int_oracle, nhwc, run_engine
+from tests.kernel_harness import DEV, IO, act_in, chan_for, out_buf, rand_act, run_both
+from tests.util import golden_act_ranges, load_net_golden, sha_i32
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 
-
-def run_both(fn_name, cpu_args, out_keys):
-    """The ABI model (tests/abi_model_mobilenetv2.py) first, then the library with every tensor in a guarded, poisoned allocation
-    (tests/util.guarded_call): outputs equal byte for byte and fully written, guards / inputs untouched, status words equal."""
-    ops.reset_status(0)
-    am.status["flags"] = 0
-    getattr(amm, fn_name)(**cpu_args)
-    outs, problems = guarded_call(getattr(ops, fn_name), cpu_args, {k: cpu_args[k] for k in out_keys}, DEV, 128 * widest_row_bytes(cpu_args))
-    assert ops.get_status(0) == am.status["flags"], (fn_name, ops.get_status(0), am.status["flags"])
-    assert not problems, (fn_name, problems)
-    return [cpu_args[k] for k in out_keys], [outs[k].cpu() for k in out_keys]
 
 # every depthwise geometry of MobileNetV2-1.0 at 224 x 224: (stored C, input H = W, stride)
 DW_GEOMS = [(64, 112, 1), (128, 112, 2), (192, 56, 1), (192, 56, 2), (192, 28, 1), (384, 28, 2), (384, 14, 1), (576, 14, 1),
             (576, 14, 2), (960, 7, 1)]
-# (a_bits, value range of the input, out_bits, clamp): int8, 4-bit values in byte containers, packed nibbles
-IO = [(8, "s8", 8, (-128, 127)), (8, "u4", 8, (0, 15)), (4, "u4", 4, (0, 15)), (8, "s8", 4, (0, 15)), (4, "u4", 8, (-128, 127))]
-
-
-def act_in(r, n_vals, kind, a_bits):
-    if a_bits == 4:
-        return rand_act(r, n_vals, 4)
-    lo, hi = (-128, 128) if kind == "s8" else (0, 16)
-    return torch.from_numpy(r.randint(lo, hi, size=n_vals).astype(np.int8))
-
-
-def chan_for(r, c, ratio_hi, clamp, caps, bias_span=3000, saturate=False):
-    """ratios in [1e-4, ratio_hi] (> 1 takes the exact requantisation); caps: 'some' bind on every third channel, 'none' = hi."""
-    me = [dyadic(float(np.exp(r.uniform(np.log(1e-4), np.log(ratio_hi))))) for _ in range(c)]
-    bias = r.randint(-bias_span, bias_span, size=c).astype(np.int64)
-    if saturate:                                           # acc + bias leaves int32 on some channels
-        bias[::5] = 2 ** 31 - 1 - r.randint(0, 1000, size=len(bias[::5]))
-        bias[1::5] = -2 ** 31 + r.randint(0, 1000, size=len(bias[1::5]))
-    lo, hi = clamp
-    cap = np.full(c, hi, dtype=np.int64)
-    if caps == "some":
-        cap[::3] = r.randint(min(max(lo, 0), hi), hi + 1, size=len(cap[::3]))
-    return ops.make_chan(bias, [m for m, _ in me], [e for _, e in me], cap)
 
 
 def dw_case(r, n, h, c, stride, io, ratio_hi=0.9, caps="some", relu=2, saturate=False, clamp=None):
@@ -145,7 +108,7 @@ def test_conv_requant_relu6_caps(geom, a_bits):
 @pytest.mark.parametrize("scheme", SCHEMES)
 def test_network_eager_and_compiled(scheme, a4_container, monkeypatch):
     monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
-    logits_g, meta = load(scheme)
+    logits_g, meta = load_net_golden("mobilenetv2_w1", scheme)
     xg = synthetic_batch(*meta["input"])
     _, _, net = int_oracle(scheme, golden_act_ranges(meta), xg)
     want = net(xg.numpy(), trace=True)

@@ -8,20 +8,14 @@ import hawq_b200 as hb
 from hawq_b200 import qtensor
 from hawq_b200.synthetic import synthetic_batch
 from oracle import int_ref as ir
-from tests.util import RESNET_GOLDENS, build_fakequant, golden_act_ranges, load_net_golden, sha_i32
+from tests.engine_harness import MIXED_WIDTH_RESIZE, check_benchmarked_configuration_matches_oracle_on_every_row, golden_model
+from tests.util import RESNET_GOLDENS, build_fakequant, load_net_golden, sha_i32
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 # every golden at a4_container 8, and packed nibbles too for the schemes with 4-bit activations
 A4_CONFIGS = [(a, s, 8) for a, s in RESNET_GOLDENS] + [(a, s, 4) for a, s in RESNET_GOLDENS
                                                        if any(v["bits"] == 4 for v in load_net_golden(a, s)[1]["acts"].values())]
-# resize units whose identity input is 4-bit and whose last convolution's input is 8-bit: with packed nibbles the two 1x1 inputs
-# have different widths, so the dual kernel is declined there (identity RAW_I32 conv + RESIDUAL conv instead)
-MIXED_WIDTH_RESIZE = {("resnet50", "modelsize_0.25"): 1, ("resnet50", "latency_0.25"): 1}
-
-
-def _model(arch, scheme, meta):
-    return hb.build_synthetic_qresnet(arch, scheme, act_ranges=golden_act_ranges(meta))
 
 
 @pytest.mark.parametrize("arch,scheme", RESNET_GOLDENS)
@@ -29,7 +23,7 @@ def _model(arch, scheme, meta):
 def test_eager_module_api_matches_golden(arch, scheme, res_bits):
     """Frozen module-by-module forward (the drop-in API) on fp32 NCHW CUDA input: logits bit-equal to the reference."""
     logits_g, meta = load_net_golden(arch, scheme)
-    q = _model(arch, scheme, meta)
+    q = golden_model(arch, scheme, meta)
     x = synthetic_batch(*meta["input"]).to(DEV)
     qtensor.config.residual_bits = res_bits
     try:
@@ -52,7 +46,7 @@ def test_every_activation_matches_oracle(arch, scheme):
     net_i = ir.IntResNet(fqm.harvest())
     li = net_i(x.numpy(), trace=True)
     assert np.array_equal(li, logits_g)
-    q = _model(arch, scheme, meta)
+    q = golden_model(arch, scheme, meta)
     rec = {}
     for name, m in q.named_modules():
         if isinstance(m, (hb.QuantAct, hb.q_resnet.QResidualUnit)):
@@ -81,7 +75,7 @@ def test_compiled_graph_int8_input_and_batch_invariance(arch, scheme, a4_contain
     The uint16 stream runs each bottleneck resize unit as one dual kernel, except where the two inputs differ in width."""
     monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
     logits_g, meta = load_net_golden(arch, scheme)
-    q = _model(arch, scheme, meta)
+    q = golden_model(arch, scheme, meta)
     B = 32
     xg = synthetic_batch(*meta["input"])
     s_in = np.float32(meta["acts"]["quant_input"]["scale"])
@@ -116,7 +110,7 @@ def test_uint16_overflow_falls_back_exactly():
     and the engine transparently re-runs with int32 residuals; the result equals the oracle."""
     arch, scheme = "resnet18", "uniform8"
     _, meta = load_net_golden(arch, scheme)
-    q = _model(arch, scheme, meta)
+    q = golden_model(arch, scheme, meta)
     # force a tiny 16-bit range so that overflow certainly happens
     for name, m in q.named_modules():
         if name.endswith("quant_act_int32") and name != "quant_act_int32":
@@ -139,7 +133,7 @@ def test_compiled_graph_uint8_pixels_equal_the_torch_pipeline():
     (transforms.ToTensor + Normalize, fp32 NCHW) fed to the same frozen model; and weights reloaded in place invalidate the plan."""
     from hawq_b200.engine import IMAGENET_MEAN, IMAGENET_STD
     logits_g, meta = load_net_golden("resnet18", "uniform8")
-    q = _model("resnet18", "uniform8", meta)
+    q = golden_model("resnet18", "uniform8", meta)
     g = torch.Generator().manual_seed(5)
     u8 = torch.randint(0, 256, (3, 224, 224, 3), generator=g, dtype=torch.uint8)
     x = u8.permute(0, 3, 1, 2).to(torch.float32).div(255)                               # transforms.ToTensor
@@ -167,38 +161,4 @@ BENCH_CONFIGS = [("resnet18", "uniform8", 8, 8), ("resnet18", "uniform4", 128, 8
 
 @pytest.mark.parametrize("arch,scheme,batch,a4_container", BENCH_CONFIGS)
 def test_benchmarked_configuration_matches_oracle_on_every_row(arch, scheme, batch, a4_container, monkeypatch, hw=224):
-    """The configuration bench.py times (CUDA graph, fused kernels, uint16 stream) at the benchmarked batch size against the
-    oracle (the reference's fake-quant forward restated on the CPU, oracle/fakequant.py): ALL rows of the logits bit-equal, and the
-    integers of the residual stream at the end of stage 1 and of the last stage (eager pass with the same kernels) equal too.
-    Many row tiles per channel block and full-size pipelines are only reached at this size.  hw: the input size (synthetic_batch)."""
-    monkeypatch.setattr(qtensor.config, "a4_container", a4_container)
-    _, meta = load_net_golden(arch, scheme)
-    x = synthetic_batch(batch, 11, hw)
-    fqm = build_fakequant(arch, scheme, meta)
-    n_stage = len(fqm.units_per_stage)
-    probes = ["stage1.unit%d.quant_act_int32" % fqm.units_per_stage[0], "stage%d.unit%d.quant_act_int32" % (n_stage, fqm.units_per_stage[-1])]
-    want_logits = fqm(x, trace=probes).numpy()
-    want = {k: np.maximum(v.numpy(), 0) for k, v in fqm.trace.items()}            # the stream is stored after the unit's ReLU
-    s_in = np.float32(meta["acts"]["quant_input"]["scale"])
-    q_in = torch.from_numpy(ir.quantize_input(x.numpy(), s_in).astype(np.int8)).to(DEV)      # NHWC int8
-    q = _model(arch, scheme, meta)
-    eng = hb.compile_model(q, q_in)
-    got = eng(q_in).cpu().numpy()
-    assert eng.fallbacks == 0
-    assert got.shape == want_logits.shape and np.array_equal(got, want_logits), \
-        "rows differing from the oracle: %s" % np.nonzero((got != want_logits).any(axis=1))[0][:16].tolist()
-    # residual-stream integers, eager pass through the same kernels
-    rec = {}
-    for name, m in q.named_modules():
-        if isinstance(m, hb.q_resnet.QResidualUnit) and (name + ".quant_act_int32") in want:
-            m.register_forward_hook(lambda mod, inp, out, name=name: rec.__setitem__(name + ".quant_act_int32", out[0]))
-    n, h, w, c = q_in.shape
-    hb.ops.reset_status(0)
-    with torch.no_grad(), qtensor.engine_mode(residual_bits=16, checked=True):
-        q(hb.IntActivation(qtensor.Node("int", (n, c, h, w), data=q_in.view(-1), bits=8, signed=True), q_in.device))
-    torch.cuda.synchronize()
-    assert hb.ops.get_status(0) & 7 == 0
-    assert set(rec) == set(want)
-    for name, t in rec.items():
-        g = t.int_tensor().cpu().numpy()
-        assert np.array_equal(g, want[name]), (name, int((g != want[name]).sum()))
+    check_benchmarked_configuration_matches_oracle_on_every_row(arch, scheme, batch, a4_container, monkeypatch, hw)

@@ -9,16 +9,12 @@ import numpy as np
 import pytest
 import torch
 
-from hawq_b200 import _lib, ops
-from hawq_b200._lib import dyadic
+from hawq_b200 import ops
+from oracle.int_ref import dyadic          # the library's (m, e) pairs, and importable without it
 from tests import abi_model as am
-from tests.test_kernels_gpu import DEV, I32_MAX, I32_MIN, RATIO_ONE, edge_biases, out_buf, rng, run_both
+from tests.kernel_harness import DEV, I32_MAX, I32_MIN, RATIO_ONE, edge_biases, kernel_count, out_buf, rng, run_both, sm_count
 
 pytestmark = pytest.mark.gpu
-
-
-def sm_count():
-    return _lib.load().hawq_sm_count(ops.handle(0))
 
 
 def stem_cta_cap():
@@ -33,10 +29,6 @@ def grid_stride_cap():
 def at_least(per_unit, items):
     """the smallest count of units of per_unit work items that reaches items"""
     return -(-items // per_unit)
-
-
-def kernel_count(family):
-    return _lib.load().hawq_debug_kernel_count(family)
 
 
 # ------------------------------------------------------------------------------------------------ stem
