@@ -73,6 +73,8 @@ SIGNATURES = {
     "hawq_avgpool_requant": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _u32, _i32, _i32, _i32, _vp, _vp]),
     "hawq_quantize_input_f32": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _f32, _i32, _i32, _vp, _vp]),
     "hawq_quantize_input_u8": (_i32, [_vp, _i32, _i32, _i32, _vp, C.POINTER(_f32), C.POINTER(_f32), _f32, _i32, _i32, _vp, _vp]),
+    "hawq_resize_crop_quantize_u8": (_i32, [_vp, _i32, _vp, _i64, _vp, _i32, _i32, _i32, C.POINTER(_f32), C.POINTER(_f32), _f32, _i32,
+                                            _i32, _vp, _vp]),
     "hawq_requant": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "hawq_add_requant": (_i32, [_vp, _i64, _i32, _vp, _vp, C.POINTER(hawq_epilogue_desc), _vp, _vp, _vp, _vp, _vp]),
     "hawq_dequant_f32": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _f32, _vp, _vp]),

@@ -10,6 +10,7 @@
 #include "conv_igemm.cuh"
 #include "conv_tail.cuh"
 #include "elementwise.cuh"
+#include "eval_transform.cuh"
 #include "mobilenet.cuh"
 #include "stem.cuh"
 
@@ -507,6 +508,26 @@ int hawq_quantize_input_u8(hawq_handle* h, int32_t N, int32_t H, int32_t W, cons
   quantize_input_u8_kernel<<<grid_for(n_bytes / 4 + 1, h->sm_count), 256, 0, (cudaStream_t)stream>>>(
       x, n_bytes, 3, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2], inv, lo, hi, out);
   return launch_check("quantize_input_u8");
+}
+
+int hawq_resize_crop_quantize_u8(hawq_handle* h, int32_t B, const uint8_t* pixels, int64_t pixel_bytes, const hawq_image_desc* table,
+                                 int32_t S, int32_t Ch, int32_t Cw, const float* mean3, const float* std3, float scale, int32_t lo,
+                                 int32_t hi, int8_t* out, void* stream) {
+  if (!h || !pixels || !table || !out || !mean3 || !std3) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: null argument");
+  if (B < 1 || B > 65535) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: B = %d outside 1..65535", B);
+  if (Ch < 1 || Cw < 1 || pixel_bytes < 0) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: empty crop or negative arena");
+  if (S < ET_MIN_RESIZE || S > ET_MAX_SIDE || S < Ch || S < Cw)
+    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_resize_crop_quantize_u8: resize %d must lie in %d..%d and cover the crop %dx%d", S,
+                ET_MIN_RESIZE, ET_MAX_SIDE, Ch, Cw);
+  if (!(scale > 0.f)) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: scale must be > 0");
+  if (lo < -128 || hi > 127 || lo > hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: clamp must fit int8");
+  for (int c = 0; c < 3; ++c)
+    if (!(std3[c] > 0.f)) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: std must be > 0");
+  const float inv = 1.0f / scale;  // as hawq_quantize_input_u8
+  const dim3 grid((Cw + ET_TW - 1) / ET_TW, (Ch + ET_TR - 1) / ET_TR, B);
+  resize_crop_quantize_u8_kernel<<<grid, ET_THREADS, 0, (cudaStream_t)stream>>>(pixels, pixel_bytes, table, S, Ch, Cw, mean3[0], mean3[1],
+                                                                                  mean3[2], std3[0], std3[1], std3[2], inv, lo, hi, out);
+  return launch_check("resize_crop_quantize_u8");
 }
 
 int hawq_requant(hawq_handle* h, int64_t rows, int32_t C, int32_t x_bits, const void* x, const hawq_chan* chan,

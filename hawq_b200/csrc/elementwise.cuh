@@ -83,14 +83,13 @@ __global__ void __launch_bounds__(256) quantize_input_kernel(const float* __rest
   }
 }
 
-// uint8 image pipeline (SURVEY.md 8(f) rank 2; tvm_benchmark/test_resnet_accuracy_imagenet.py:62-75,82-93): ToTensor (u / 255),
-// Normalize ((v - mean_c) / std_c) and the QuantAct input branch (clamp(rint((1/scale) * x))) in one pass, uint8 NHWC -> int8 NHWC.
-// Every step is the same single fp32 operation the reference's torch pipeline performs, so the integers are identical; with
-// 256 possible inputs per channel the whole map is a 3 x 256 table built once per block in shared memory.
-__global__ void __launch_bounds__(256) quantize_input_u8_kernel(const uint8_t* __restrict__ x, long long n_bytes, int C,
-                                                                float m0, float m1, float m2, float s0, float s1, float s2,
-                                                                float inv_scale, int lo, int hi, int8_t* __restrict__ out) {
-  __shared__ int8_t lut[3 * 256];
+// uint8 pixel -> int8 network input table of the uint8 image pipelines (SURVEY.md 8(f) rank 2;
+// tvm_benchmark/test_resnet_accuracy_imagenet.py:62-75,82-93): ToTensor (u / 255), Normalize ((v - mean_c) / std_c) and the QuantAct
+// input branch (clamp(rint((1/scale) * x))).  Every step is the same single fp32 operation the reference's torch pipeline performs,
+// so the integers are identical; with 256 possible inputs per channel the whole map is a 3 x 256 table, lut[c << 8 | u], built by
+// the calling block in shared memory (the caller synchronises before reading it).
+__device__ __forceinline__ void build_input_lut(int8_t* lut, float m0, float m1, float m2, float s0, float s1, float s2, float inv_scale,
+                                                int lo, int hi) {
   for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) {
     const int c = i >> 8, u = i & 255;
     const float mean = c == 0 ? m0 : (c == 1 ? m1 : m2), sd = c == 0 ? s0 : (c == 1 ? s1 : s2);
@@ -98,6 +97,14 @@ __global__ void __launch_bounds__(256) quantize_input_u8_kernel(const uint8_t* _
     const float q = rintf(__fmul_rn(inv_scale, v));
     lut[i] = (int8_t)(int)fminf(fmaxf(q, (float)lo), (float)hi);
   }
+}
+
+// uint8 NHWC -> int8 NHWC through the build_input_lut table, one pass.
+__global__ void __launch_bounds__(256) quantize_input_u8_kernel(const uint8_t* __restrict__ x, long long n_bytes, int C,
+                                                                float m0, float m1, float m2, float s0, float s1, float s2,
+                                                                float inv_scale, int lo, int hi, int8_t* __restrict__ out) {
+  __shared__ int8_t lut[3 * 256];
+  build_input_lut(lut, m0, m1, m2, s0, s1, s2, inv_scale, lo, hi);
   __syncthreads();
   const long long words = n_bytes >> 2;
   for (long long wi = blockIdx.x * (long long)blockDim.x + threadIdx.x; wi < words; wi += (long long)gridDim.x * blockDim.x) {

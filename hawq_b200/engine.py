@@ -22,6 +22,7 @@ import threading
 import torch
 
 from . import ops, qtensor
+from .eval_transform import MAX_SIDE, MIN_RESIZE, PackedImages, collate_images
 from .modules import freeze_model
 from .qtensor import IntActivation, Node
 
@@ -35,10 +36,15 @@ IMAGENET_STD = (0.229, 0.224, 0.225)       # tvm_benchmark/test_resnet_accuracy_
 class CompiledModel:
     """input: int8 NHWC [N,H,W,3] (already quantised with the model's input scale), fp32 NCHW [N,3,H,W] (normalised, what the
     reference's loaders produce), or uint8 NHWC [N,H,W,3] raw pixels (ToTensor + Normalize(mean, std) + input quantisation are
-    then one kernel at the head of the graph; needs ``model.quant_input``)."""
+    then one kernel at the head of the graph; needs ``model.quant_input``).
+
+    With ``resize`` (the reference's evaluation transform, Resize(resize) -> CenterCrop(H, W) -> ToTensor -> Normalize): the input
+    is a batch of up to N decoded RGB images of any sizes, a ``PackedImages`` or a list of HWC uint8 images, and the head kernel
+    resizes, crops and quantises them on the device, bit-equal to torchvision on PIL.  The pixels go to a device arena (with a table
+    of offsets and sizes) that the graphs read; a batch that does not fit grows it and recaptures the graphs (``recaptures``)."""
 
     def __init__(self, model, example, use_cuda_graph=True, residual_bits=16, mean=IMAGENET_MEAN, std=IMAGENET_STD, gather=False,
-                 group=None):
+                 group=None, resize=None):
         if not example.is_cuda:
             raise RuntimeError("compile_model needs a CUDA example input: the frozen path has no CPU implementation")
         self.model = model
@@ -46,6 +52,9 @@ class CompiledModel:
         self.int_input = example.dtype == torch.int8
         self.u8_input = example.dtype == torch.uint8
         self.mean, self.std = tuple(mean), tuple(std)
+        self.recaptures = 0
+        if resize is not None and gather:
+            raise NotImplementedError("resize with gather=True (sharded ragged batches) is not supported")
         if self.u8_input:
             if example.dim() != 4 or example.shape[-1] != 3:
                 raise ValueError("uint8 input must be NHWC with 3 channels")
@@ -53,7 +62,18 @@ class CompiledModel:
             if act is None or act.activation_bit != 8 or act.quant_mode != "symmetric":
                 raise NotImplementedError("uint8 input needs an 8-bit symmetric `quant_input` QuantAct at the head of the model")
             self._q_in = torch.empty(example.numel(), dtype=torch.int8, device=example.device)
-        self.static_in = example.clone()
+        self.resize = None if resize is None else int(resize)
+        if self.resize is not None:
+            if not self.u8_input:
+                raise ValueError("resize needs a uint8 NHWC example: its H x W is the crop, its batch the number of image slots")
+            self.slots, self.crop = example.shape[0], (example.shape[1], example.shape[2])
+            if not MIN_RESIZE <= self.resize <= MAX_SIDE or self.resize < max(self.crop):
+                raise ValueError("resize %d must lie in %d..%d and cover the crop %dx%d" % ((self.resize, MIN_RESIZE, MAX_SIDE) + self.crop))
+            # the arena starts with room for 3 * resize^2 pixels per slot: a batch of ImageNet-sized images (500 x 375) fits
+            self.arena = torch.zeros(self.slots * 3 * self.resize * self.resize * 3, dtype=torch.uint8, device=example.device)
+            self.table = torch.zeros((self.slots, 2), dtype=torch.int64, device=example.device)   # hawq_image_desc rows; h = 0: absent
+            self._n = self.slots
+        self.static_in = example.clone() if self.resize is None else None
         self.use_graph = use_cuda_graph
         self.flag = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.gather, self.group = bool(gather), group
@@ -84,7 +104,12 @@ class CompiledModel:
 
     def _forward_checked(self):
         x = self.static_in
-        if self.u8_input:
+        if self.resize is not None:
+            act = self.model.quant_input
+            ops.resize_crop_quantize_u8(self.arena, self.table, self.resize, self.crop, self.mean, self.std, float(qtensor._frozen_scale(act)),
+                                        qtensor._act_clamp(act), self._q_in)
+            x = IntActivation(Node("int", (self.slots, 3) + self.crop, data=self._q_in, bits=8, signed=True), self.device)
+        elif self.u8_input:
             act = self.model.quant_input
             ops.quantize_input_u8(x, self.mean, self.std, float(qtensor._frozen_scale(act)), qtensor._act_clamp(act), self._q_in)
             n, h, w, c = x.shape
@@ -163,16 +188,49 @@ class CompiledModel:
     def _result(self, key):
         return self.gathered[key] if self.gather else self.outs[key]
 
+    def _grow(self, nbytes):
+        """A bigger arena for a batch of ``nbytes`` pixel bytes: every graph is recaptured over it."""
+        torch.cuda.synchronize(self.device)                  # no replay still reads the old arena
+        self.arena = torch.zeros(nbytes * 5 // 4, dtype=torch.uint8, device=self.device)
+        keys = list(self.outs)
+        self.graphs.clear()
+        with torch.no_grad():
+            for key in keys:
+                self._build(self.bits_of[key], key=key)
+        self.recaptures += 1
+
+    def _packed(self, images):
+        p = images if isinstance(images, PackedImages) else collate_images(list(images))
+        if len(p) > self.slots:
+            raise ValueError("%d images for %d slots" % (len(p), self.slots))
+        if p.pixels.numel() > self.arena.numel():
+            self._grow(p.pixels.numel())
+        return p
+
+    def _stage(self, images):
+        p = self._packed(images)
+        self.arena[:p.pixels.numel()].copy_(p.pixels, non_blocking=True)
+        self.table.copy_(p.table(self.slots), non_blocking=True)
+        self._n = len(p)
+
     def run_async(self, x=None):
         """Enqueue one forward (no host sync, no overflow check); returns the static logits tensor (with ``gather`` the logits
-        of the whole sharded batch, gathered from every rank inside the same CUDA graph)."""
-        if x is not None:
+        of the whole sharded batch, gathered from every rank inside the same CUDA graph; with ``resize`` all N rows, the rows past
+        the batch's images belonging to absent slots)."""
+        if x is not None and self.resize is not None:
+            self._stage(x)
+        elif x is not None:
             self.static_in.copy_(x, non_blocking=True)
         out = self._run(self.residual_bits)
         return self.gathered[self.residual_bits] if self.gather else out
 
     def __call__(self, x=None):
-        """Exact forward: replays the fast graph, checks the overflow flag, falls back to int32 residuals if needed."""
+        """Exact forward: replays the fast graph, checks the overflow flag, falls back to int32 residuals if needed.  With ``resize``
+        the logits of the batch's n images, [n, classes]."""
+        out = self._call(x)
+        return out if self.resize is None else out[:self._n]
+
+    def _call(self, x):
         out = self.run_async(x)
         self._last_key = self.residual_bits
         flags = self._flags()
@@ -201,7 +259,9 @@ class CompiledModel:
         copy stream while batch i computes; logits and the status flags come back through pinned buffers and are checked one
         step later (a raised overflow flag re-runs that batch through ``__call__``, i.e. the exact int32 / saturating graphs).
         ``post`` is applied to the device logits before they are read back.  With ``gather`` the logits of the whole sharded batch
-        stay on the device (``self.gathered``) and the host reads this rank's shard.
+        stay on the device (``self.gathered``) and the host reads this rank's shard.  With ``resize`` a batch is a ``PackedImages``
+        (pinned, for a copy that overlaps) or a list of images, and its rows are those of its images; the staging buffers grow
+        with the arena.
         Yields the host logits tensor of every batch, in order (valid until the second next iteration)."""
         dev = self.device
         main = torch.cuda.current_stream(dev)
@@ -212,7 +272,9 @@ class CompiledModel:
                 out = post(out)
             # three host logits buffers: batch i's is yielded during iteration i + 1 and must survive iteration i + 2, which
             # already enqueues the read-back of batch i + 2
-            self._pipe = dict(copy=cs, stage=[torch.empty_like(self.static_in) for _ in range(2)],
+            src = self.static_in if self.resize is None else self.arena
+            self._pipe = dict(copy=cs, stage=[torch.empty_like(src) for _ in range(2)],
+                              table=[torch.empty_like(self.table) for _ in range(2)] if self.resize is not None else None,
                               out=[torch.empty(out.shape, dtype=out.dtype).pin_memory() for _ in range(3)],
                               flag=[torch.zeros(self.all_flags.numel() if self.gather else 1, dtype=torch.int32).pin_memory() for _ in range(2)],
                               h2d=[torch.cuda.Event() for _ in range(2)], free=[torch.cuda.Event() for _ in range(2)],
@@ -220,22 +282,38 @@ class CompiledModel:
         P = self._pipe
         prev = None
 
-        def finish(slot, oslot, xb):
+        def finish(slot, oslot, xb, n):
             P["done"][slot].synchronize()
             if self._flags(P["flag"][slot].tolist()) & 7:
                 self(xb)                            # rare: exact fallback path, synchronous (sharded runs: every rank takes it together)
                 out = self.outs[self._last_key]
-                return (post(out) if post is not None else out).to("cpu")
-            return P["out"][oslot]
+                return (post(out) if post is not None else out).to("cpu")[:n]
+            return P["out"][oslot][:n]
 
         for i, xb in enumerate(host_batches):
             slot, oslot = i & 1, i % 3
+            n = None
+            if self.resize is not None:
+                xb = self._packed(xb)
+                n, nb = len(xb), xb.pixels.numel()
+                if nb > P["stage"][0].numel():
+                    torch.cuda.synchronize(dev)     # neither stage buffer is still being copied
+                    P["stage"] = [torch.empty_like(self.arena) for _ in range(2)]
             with torch.cuda.stream(P["copy"]):
                 P["copy"].wait_event(P["free"][slot])
-                P["stage"][slot].copy_(xb, non_blocking=True)
+                if self.resize is None:
+                    P["stage"][slot].copy_(xb, non_blocking=True)
+                else:
+                    P["stage"][slot][:nb].copy_(xb.pixels, non_blocking=True)
+                    P["table"][slot].copy_(xb.table(self.slots), non_blocking=True)
                 P["h2d"][slot].record(P["copy"])
             main.wait_event(P["h2d"][slot])
-            self.static_in.copy_(P["stage"][slot], non_blocking=True)
+            if self.resize is None:
+                self.static_in.copy_(P["stage"][slot], non_blocking=True)
+            else:
+                self.arena[:nb].copy_(P["stage"][slot][:nb], non_blocking=True)
+                self.table.copy_(P["table"][slot], non_blocking=True)
+                self._n = n
             P["free"][slot].record(main)
             out = self._run(self.residual_bits)
             if post is not None:
@@ -245,7 +323,7 @@ class CompiledModel:
             P["done"][slot].record(main)
             if prev is not None:
                 yield finish(*prev)
-            prev = (slot, oslot, xb)
+            prev = (slot, oslot, xb, n)
         if prev is not None:
             yield finish(*prev)
 
@@ -254,14 +332,17 @@ class CompiledModel:
         return self.launches.get(self.residual_bits, 0)
 
 
-def compile_model(model, example, use_cuda_graph=True, residual_bits=16, mean=IMAGENET_MEAN, std=IMAGENET_STD, gather=False, group=None):
+def compile_model(model, example, use_cuda_graph=True, residual_bits=16, mean=IMAGENET_MEAN, std=IMAGENET_STD, gather=False, group=None,
+                  resize=None):
     """Freeze ``model`` (a QResNet or any graph built from hawq_b200.modules) and compile it for ``example``'s shape and dtype
     (int8 NHWC, fp32 NCHW or uint8 NHWC; ``mean`` / ``std`` only matter for uint8 pixels).  ``gather``: the batch is sharded over the
-    ranks of ``group`` (torch.distributed, NCCL) and every forward all-gathers the logits inside the CUDA graph."""
+    ranks of ``group`` (torch.distributed, NCCL) and every forward all-gathers the logits inside the CUDA graph.  ``resize``: with a
+    uint8 NHWC example [N, H, W, 3], the engine takes up to N decoded images of any sizes and applies Resize(resize) + CenterCrop(H, W)
+    on the device (see CompiledModel)."""
     freeze_model(model)
     model.eval()
     return CompiledModel(model, example, use_cuda_graph=use_cuda_graph, residual_bits=residual_bits, mean=mean, std=std, gather=gather,
-                         group=group)
+                         group=group, resize=resize)
 
 
 def all_gather_logits(local_logits, group=None):

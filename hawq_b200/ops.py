@@ -312,6 +312,27 @@ def quantize_input_u8(x, mean, std, scale, clamp, out):
             label="quantize_input_u8", work=lambda: (0, n * hh * ww * 6))
 
 
+def resize_crop_quantize_u8(pixels, table, size, crop, mean, std, scale, clamp, out):
+    """Ragged uint8 HWC images -> int8 NHWC [B, Ch, Cw, 3] network input: Resize(size) + CenterCrop(crop) (torchvision on PIL, bit for
+    bit) + ToTensor + Normalize + QuantAct input branch in one kernel.  pixels: the uint8 arena; table: int64 [B, 2] hawq_image_desc
+    rows (eval_transform.PackedImages.table) on the device.  Timer work: the source bytes the crops read plus the output bytes."""
+    ch, cw = crop
+    b = table.shape[0]
+    m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+
+    def work():
+        from .eval_transform import source_box
+        t = table.cpu()
+        read = 0
+        for off, h, w in zip(t[:, 0].tolist(), t.view(torch.int32)[:, 2].tolist(), t.view(torch.int32)[:, 3].tolist()):
+            if h > 0:
+                (_, rows), (_, cols) = source_box(h, w, size, crop)
+                read += rows * cols * 3
+        return 0, read + b * ch * cw * 3
+    _launch(pixels, "hawq_resize_crop_quantize_u8", b, _p(pixels), pixels.numel(), _p(table), size, ch, cw, m3, s3, float(scale), clamp[0],
+            clamp[1], _p(out), label="resize_crop_quantize_u8", work=work)
+
+
 def requant(x, rows, c, x_bits, chan, chan_stride, relu, out_bits, clamp, out):
     _launch(x, "hawq_requant", rows, c, x_bits, _p(x), _p(chan), chan_stride, int(relu), out_bits, clamp[0], clamp[1], _p(out))
 

@@ -221,6 +221,23 @@ int hawq_quantize_input_f32(hawq_handle* h, int32_t N, int32_t C, int32_t H, int
  * operation as in the torch pipeline.  mean3 / std3 are HOST pointers to three floats (copied at launch). */
 int hawq_quantize_input_u8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const uint8_t* x, const float* mean3,
                            const float* std3, float scale, int32_t lo, int32_t hi, int8_t* out, void* stream);
+
+/* One image of a ragged batch: h x w x 3 uint8 pixels (HWC) at byte `offset` of the pixel arena.  h == 0: an absent slot. */
+typedef struct {
+  int64_t offset;
+  int32_t h, w;
+} hawq_image_desc;
+
+/* The reference's evaluation transform (quant_train.py:427-438): Resize(S) -> CenterCrop(Ch, Cw) -> ToTensor -> Normalize ->
+ * QuantAct input branch, for B images of any size in one launch.  table: DEVICE array of B hawq_image_desc into the DEVICE pixel
+ * arena `pixels` of `pixel_bytes` bytes; out: int8 NHWC [B, Ch, Cw, 3].  The resize and crop are torchvision's on PIL images,
+ * bit for bit (bilinear, 8 bits per channel); the last three steps are hawq_quantize_input_u8's table.  Every per-image quantity is
+ * computed on the device, so the launch depends only on B, Ch and Cw (a captured graph serves any image sizes).  Requirements:
+ * 256 <= S <= 16384, S >= max(Ch, Cw), 1 <= B <= 65535.  An entry with h == 0, a side outside 1..16384 or pixels outside the arena
+ * is absent: its output is the quantised zero pixel.  mean3 / std3 are HOST pointers to three floats (copied at launch). */
+int hawq_resize_crop_quantize_u8(hawq_handle* h, int32_t B, const uint8_t* pixels, int64_t pixel_bytes, const hawq_image_desc* table,
+                                 int32_t S, int32_t Ch, int32_t Cw, const float* mean3, const float* std3, float scale, int32_t lo,
+                                 int32_t hi, int8_t* out, void* stream);
 /* fixedpoint_fn case 0 stand-alone (QuantAct after a conv or at unit entry): x [rows,C] (x_bits 16 = uint16 residual,
  * 32 = int32), per-channel chan (bias is added; pass 0) or scalar when chan_stride == 0 (chan[0] used for all). */
 int hawq_requant(hawq_handle* h, int64_t rows, int32_t C, int32_t x_bits, const void* x, const hawq_chan* chan,
