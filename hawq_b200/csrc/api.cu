@@ -156,6 +156,71 @@ int hawq_copy_status(hawq_handle* h, int32_t* dst, void* stream) {
   return HAWQ_OK;
 }
 
+// ------------------------------------------------------------------------------------------- argument checks
+// Each returns HAWQ_OK or the entry point's error; fn, the entry point's name, prefixes the message.
+static int check_me(const char* fn, const char* what, uint32_t m, int e) {
+  return e < 1 || e > 62 || m > 0x80000000u ? fail(HAWQ_ERR_BAD_ARG, "%s: %s dyadic pair out of range (m=%u e=%d)", fn, what, m, e) : HAWQ_OK;
+}
+
+static int out_size(int in, int k, int stride, int pad) { return (in + 2 * pad - k) / stride + 1; }
+
+// The descriptor of a wgmma convolution; bn: the channel block of the launch's output tiles
+static int check_conv_desc(const char* fn, const hawq_conv_desc* d, int bn) {
+  if (d->N < 1 || d->H < 1 || d->W < 1 || d->kh < 1 || d->kw < 1 || d->stride < 1 || d->pad < 0) return fail(HAWQ_ERR_BAD_ARG, "%s: bad geometry", fn);
+  if (d->a_bits != 8 && d->a_bits != 4) return fail(HAWQ_ERR_UNSUPPORTED, "%s: a_bits must be 4 or 8", fn);
+  if (d->Cin % 64 != 0 || d->Cout % 64 != 0) return fail(HAWQ_ERR_UNSUPPORTED, "%s: Cin (%d) and Cout (%d) must be multiples of 64", fn, d->Cin, d->Cout);
+  if (d->Cin < 64 || d->Cout < 64) return fail(HAWQ_ERR_BAD_ARG, "%s: Cin (%d) and Cout (%d) must be at least 64", fn, d->Cin, d->Cout);
+  const int Ho = out_size(d->H, d->kh, d->stride, d->pad), Wo = out_size(d->W, d->kw, d->stride, d->pad);
+  if (Ho < 1 || Wo < 1) return fail(HAWQ_ERR_BAD_ARG, "%s: empty output", fn);
+  const long long M = (long long)d->N * Ho * Wo;
+  if (M > 0x7fffff00ll || (long long)d->N * d->H * d->W > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "%s: too many pixels", fn);
+  if ((M + CONV_BM - 1) / CONV_BM * (d->Cout / bn) > 0x7fffffffll) return fail(HAWQ_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 output tiles", fn);
+  return HAWQ_OK;
+}
+
+// The tensors of a direct kernel: at least one image, channel, and row and column (min_side where a stem's window must fit)
+static int check_dims(const char* fn, int N, int H, int W, int C, int min_side = 1) {
+  return N < 1 || H < min_side || W < min_side || C < 1 ? fail(HAWQ_ERR_BAD_ARG, "%s: bad geometry", fn) : HAWQ_OK;
+}
+
+// The launch of a direct kernel: input pixel offsets inside int32, at most 2^31 - 1 CTAs
+static int check_limits(const char* fn, long long pixels, long long ctas) {
+  if (pixels > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "%s: too many pixels", fn);
+  if (ctas > 0x7fffffffll) return fail(HAWQ_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 CTAs", fn);
+  return HAWQ_OK;
+}
+
+// A clamp range: not empty, and inside int8 / int16 where `bits` names the stored type
+static int check_clamp(const char* fn, int lo, int hi, int bits = 0) {
+  if (lo > hi) return fail(HAWQ_ERR_BAD_ARG, "%s: empty clamp range", fn);
+  if (bits && (lo < -(1 << (bits - 1)) || hi >= 1 << (bits - 1))) return fail(HAWQ_ERR_BAD_ARG, "%s: clamp must fit int%d", fn, bits);
+  return HAWQ_OK;
+}
+
+// The low-bit copy clamp(RHE(y * low_m / 2^low_e), low_lo, low_hi): none (low_bits 0), int8 or packed nibbles in out_low
+static int check_low(const char* fn, int low_bits, uint32_t low_m, int low_e, const void* out_low) {
+  if (low_bits != 0 && low_bits != 4 && low_bits != 8) return fail(HAWQ_ERR_BAD_ARG, "%s: low_bits must be 0/4/8", fn);
+  if (!low_bits) return HAWQ_OK;
+  if (!out_low) return fail(HAWQ_ERR_BAD_ARG, "%s: low_bits set but out_low is null", fn);
+  return check_me(fn, "low-bit copy", low_m, low_e);
+}
+
+// The RESIDUAL operand and outputs of an epilogue
+static int check_residual(const char* fn, const hawq_epilogue_desc* ep, const void* res, const hawq_chan* res_chan, const void* y,
+                          const void* out_low) {
+  if (!res) return fail(HAWQ_ERR_BAD_ARG, "%s: RESIDUAL needs res", fn);
+  if (ep->res_kind != 0 && ep->res_kind != 1) return fail(HAWQ_ERR_BAD_ARG, "%s: res_kind must be 0/1", fn);
+  if (ep->res_kind == 1 && !res_chan) return fail(HAWQ_ERR_BAD_ARG, "%s: res_kind 1 needs res_chan", fn);
+  if (ep->res_kind == 0 && ep->res_bits != 16 && ep->res_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "%s: res_bits must be 16/32", fn);
+  if (int rc = ep->res_kind == 0 ? check_me(fn, "residual", ep->res_m, ep->res_e) : HAWQ_OK) return rc;
+  if (ep->y_bits != 0 && ep->y_bits != 16 && ep->y_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "%s: y_bits must be 0/16/32", fn);
+  if (ep->y_bits == 16 && !ep->relu) return fail(HAWQ_ERR_BAD_ARG, "%s: uint16 residual stream requires relu", fn);
+  if (ep->y_bits && !y) return fail(HAWQ_ERR_BAD_ARG, "%s: y_bits set but the stream pointer is null", fn);
+  if (!ep->y_bits && !ep->low_bits) return fail(HAWQ_ERR_BAD_ARG, "%s: RESIDUAL with no output", fn);
+  return check_low(fn, ep->low_bits, ep->low_m, ep->low_e, out_low);
+}
+
+// ------------------------------------------------------------------------------------------- kernel parameters
 // |acc| <= K * 128 * 128 (int8 activations) or K * 15 * 128 (unsigned 4-bit activations), int8 weights: a bias in
 // [bias_lo, bias_hi] keeps acc + bias inside int32, so the FP64 epilogue needs no clamp
 static void set_bias_window(ConvParams& p, int a_bits) {
@@ -165,73 +230,54 @@ static void set_bias_window(ConvParams& p, int a_bits) {
   p.bias_hi = (int)(2147483647ll - bound);
 }
 
-static int check_me(uint32_t m, int e, const char* what) {
-  if (e < 1 || e > 62 || m > 0x80000000u) return fail(HAWQ_ERR_BAD_ARG, "%s: dyadic pair out of range (m=%u e=%d)", what, m, e);
-  return HAWQ_OK;
+// Zeroed parameters of the convolution d with its pointers, geometry and bias window.  K counts the products of one output:
+// kh * kw * Cin, or kh * kw in a depthwise convolution (one input channel per output channel).
+static ConvParams conv_params(const hawq_handle* h, const hawq_conv_desc& d, const void* x, const int8_t* w, const hawq_chan* chan,
+                              void* out, bool depthwise = false) {
+  ConvParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = out; p.status = h->status;
+  p.N = d.N; p.H = d.H; p.W = d.W; p.Cin = d.Cin; p.Cout = d.Cout; p.KH = d.kh; p.KW = d.kw; p.stride = d.stride; p.pad = d.pad;
+  p.Ho = out_size(d.H, d.kh, d.stride, d.pad); p.Wo = out_size(d.W, d.kw, d.stride, d.pad);
+  p.M = (int)((long long)d.N * p.Ho * p.Wo); p.K = d.kh * d.kw * (depthwise ? 1 : d.Cin);
+  p.cin_chunks = d.Cin / 64; p.x_pix_bytes = d.Cin * d.a_bits / 8;
+  set_bias_window(p, d.a_bits);
+  return p;
 }
+
+// Copies the epilogue into p and derives the scalar part of the kernel's requantisation policy (load_channel_block): whether the scalar
+// ratio of a res_kind 0 residual operand or of the low-bit copy exceeds 1 or 2^20, and whether RESIDUAL terms leaving int32 are flagged
+// (under a ratio promise).  writes_low: the kernel writes the low-bit copy (RESIDUAL kernels, the stems; not hawq_conv2d's other modes).
+static void set_epilogue(ConvParams& p, const hawq_epilogue_desc& ep, bool writes_low) {
+  p.mode = ep.mode; p.relu = ep.relu; p.out_bits = ep.out_bits; p.lo = ep.clamp_lo; p.hi = ep.clamp_hi;
+  p.res_kind = ep.res_kind; p.res_bits = ep.res_bits; p.res_m = ep.res_m; p.res_e = ep.res_e;
+  p.y_bits = ep.y_bits; p.low_bits = ep.low_bits; p.low_m = ep.low_m; p.low_e = ep.low_e; p.low_lo = ep.low_lo; p.low_hi = ep.low_hi;
+  p.cout_store = ep.cout_store;
+  const bool residual = ep.mode == HAWQ_EPI_RESIDUAL, scalar_res = residual && ep.res_kind == 0;
+  const bool low_over_one = writes_low && ep.low_bits != 0 && !dyadic_is_fast(ep.low_m, ep.low_e);
+  p.scalar_over_one = (scalar_res && !dyadic_is_fast(ep.res_m, ep.res_e)) || low_over_one;
+  p.scalar_unchecked = (scalar_res && !dyadic_is_wide(ep.res_m, ep.res_e)) || low_over_one;
+  p.check_ovf = residual && (ep.flags & (HAWQ_EP_RATIOS_LE_ONE | HAWQ_EP_RATIOS_LE_2P20)) != 0;
+}
+
+// persistent kernels: 4 CTAs per SM loop over the tiles and stage the weights once (round-2 A/B: 0.212 -> 0.202 ms at batch 128)
+static int persistent_ctas(long long tiles, int sm_count) { return (int)(tiles < 4LL * sm_count ? tiles : 4LL * sm_count); }
 
 int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_desc* ep, const void* x, const int8_t* w,
                 const hawq_chan* chan, const void* res, const hawq_chan* res_chan, const float* fscale, void* out,
                 void* out_low, void* stream) {
   if (!h || !d || !ep || !x || !w || !chan) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: null argument");
-  if (d->N < 1 || d->H < 1 || d->W < 1 || d->kh < 1 || d->kw < 1 || d->stride < 1 || d->pad < 0)
-    return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: bad geometry");
-  if (d->a_bits != 8 && d->a_bits != 4) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: a_bits must be 4 or 8");
-  if (d->Cin % 64 != 0 || d->Cout % 64 != 0)
-    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: Cin (%d) and Cout (%d) must be multiples of 64", d->Cin, d->Cout);
-  if (d->Cin < 64 || d->Cout < 64) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: Cin (%d) and Cout (%d) must be at least 64", d->Cin, d->Cout);
-  const int Ho = (d->H + 2 * d->pad - d->kh) / d->stride + 1;
-  const int Wo = (d->W + 2 * d->pad - d->kw) / d->stride + 1;
-  if (Ho < 1 || Wo < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: empty output");
-  const long long M = (long long)d->N * Ho * Wo;
-  if (M > 0x7fffff00ll || (long long)d->N * d->H * d->W > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: too many pixels");
-
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.res = res; p.res_chan = res_chan; p.fscale = fscale;
-  p.out = out; p.out_low = out_low; p.status = h->status;
-  p.N = d->N; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout; p.KH = d->kh; p.KW = d->kw;
-  p.stride = d->stride; p.pad = d->pad; p.Ho = Ho; p.Wo = Wo; p.M = (int)M; p.K = d->kh * d->kw * d->Cin;
-  p.cin_chunks = d->Cin / 64;
-  p.x_pix_bytes = d->Cin * d->a_bits / 8;
-  p.mode = ep->mode; p.relu = ep->relu; p.out_bits = ep->out_bits; p.lo = ep->clamp_lo; p.hi = ep->clamp_hi;
-  p.res_kind = ep->res_kind; p.res_bits = ep->res_bits; p.res_m = ep->res_m; p.res_e = ep->res_e;
-  p.y_bits = ep->y_bits; p.low_bits = ep->low_bits; p.low_m = ep->low_m; p.low_e = ep->low_e;
-  p.low_lo = ep->low_lo; p.low_hi = ep->low_hi; p.cout_store = ep->cout_store;
-  set_bias_window(p, d->a_bits);
-  p.check_ovf = ep->mode == HAWQ_EPI_RESIDUAL && (ep->flags & (HAWQ_EP_RATIOS_LE_ONE | HAWQ_EP_RATIOS_LE_2P20)) != 0;
-  if (ep->mode == HAWQ_EPI_RESIDUAL) {   // the scalar ratios' part of the kernel's per-CTA requantisation policy
-    const bool low_over_one = ep->low_bits != 0 && !dyadic_is_fast(ep->low_m, ep->low_e);
-    p.scalar_over_one = (ep->res_kind == 0 && !dyadic_is_fast(ep->res_m, ep->res_e)) || low_over_one;
-    p.scalar_unchecked = (ep->res_kind == 0 && !dyadic_is_wide(ep->res_m, ep->res_e)) || low_over_one;
-  }
-
+  const bool bn128 = (d->Cout % 128 == 0);
+  if (int rc = check_conv_desc(__func__, d, bn128 ? 128 : 64)) return rc;
   switch (ep->mode) {
     case HAWQ_EPI_REQUANT:
       if (!out) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: REQUANT needs out");
       if (ep->out_bits != 4 && ep->out_bits != 8 && ep->out_bits != 16 && ep->out_bits != 32)
         return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: out_bits must be 4/8/16/32");
-      if (ep->clamp_lo > ep->clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: empty clamp range");
+      if (int rc = check_clamp(__func__, ep->clamp_lo, ep->clamp_hi)) return rc;
       break;
     case HAWQ_EPI_RESIDUAL:
-      if (!res) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: RESIDUAL needs res");
-      if (ep->res_kind == 1) {
-        if (!res_chan) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: res_kind 1 needs res_chan");
-      } else if (ep->res_kind == 0) {
-        if (ep->res_bits != 16 && ep->res_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: res_bits must be 16/32");
-        int rc = check_me(ep->res_m, ep->res_e, "hawq_conv2d residual");
-        if (rc) return rc;
-      } else return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: res_kind must be 0/1");
-      if (ep->y_bits != 0 && ep->y_bits != 16 && ep->y_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: y_bits must be 0/16/32");
-      if (ep->y_bits == 16 && !ep->relu) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: uint16 residual stream requires relu");
-      if (ep->y_bits && !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: y_bits set but out is null");
-      if (ep->low_bits != 0 && ep->low_bits != 4 && ep->low_bits != 8) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: low_bits must be 0/4/8");
-      if (ep->low_bits) {
-        if (!out_low) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: low_bits set but out_low is null");
-        int rc = check_me(ep->low_m, ep->low_e, "hawq_conv2d low-bit copy");
-        if (rc) return rc;
-      }
-      if (!ep->y_bits && !ep->low_bits) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: RESIDUAL with no output");
+      if (int rc = check_residual(__func__, ep, res, res_chan, out, out_low)) return rc;
       break;
     case HAWQ_EPI_RAW_I32:
       if (!out) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: RAW_I32 needs out");
@@ -244,9 +290,9 @@ int hawq_conv2d(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogue_des
       return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d: unknown epilogue mode %d", ep->mode);
   }
 
-  const bool bn128 = (d->Cout % 128 == 0);
-  if ((M + CONV_BM - 1) / CONV_BM * (d->Cout / (bn128 ? 128 : 64)) > 0x7fffffffll)
-    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d: more than 2^31 - 1 output tiles");
+  ConvParams p = conv_params(h, *d, x, w, chan, out);
+  p.res = res; p.res_chan = res_chan; p.fscale = fscale; p.out_low = out_low;
+  set_epilogue(p, *ep, ep->mode == HAWQ_EPI_RESIDUAL);
   ++g_kernel_count[0];
   cudaStream_t s = (cudaStream_t)stream;
   // bottleneck tails (1x1 stride 1, uint16 residual operand and stream): the persistent tail kernel
@@ -274,41 +320,25 @@ int hawq_conv2d_dual(hawq_handle* h, const hawq_conv_desc* d, const hawq_epilogu
   if (!h || !d || !ep || !x || !w || !chan || !d2 || !x2 || !w2 || !chan2 || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: null argument");
   if (d->kh != 1 || d->kw != 1 || d->stride != 1 || d->pad != 0 || d2->kh != 1 || d2->kw != 1 || d2->pad != 0 || d2->stride < 1)
     return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: both convolutions must be 1x1 without padding (main stride 1)");
-  if (d->N < 1 || d->H < 1 || d->W < 1 || d2->H < 1 || d2->W < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: bad geometry");
-  if ((d->a_bits != 8 && d->a_bits != 4) || d2->a_bits != d->a_bits) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: a_bits must be equal and 4 or 8");
-  if (d->Cin % 64 || d2->Cin % 64 || d->Cout % 64 || d2->Cout != d->Cout) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: channel counts must be multiples of 64 and Cout equal");
-  if (d->Cin < 64 || d2->Cin < 64 || d->Cout < 64) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: Cin and Cout must be at least 64");
-  if (d2->N != d->N || (d2->H - 1) / d2->stride + 1 != d->H || (d2->W - 1) / d2->stride + 1 != d->W)
+  int rc;
+  if ((rc = check_conv_desc(__func__, d, 64))) return rc;
+  if (d2->a_bits != d->a_bits || d2->Cout != d->Cout) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: a_bits and Cout must be equal");
+  if (d2->N != d->N || out_size(d2->H, 1, d2->stride, 0) != d->H || out_size(d2->W, 1, d2->stride, 0) != d->W)
     return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: the two convolutions have different output grids");
+  if ((rc = check_conv_desc(__func__, d2, 64))) return rc;
   if (d->w_layout != 1 || d2->w_layout != 1) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: weights must carry the re-tiled copy (w_layout 1)");
   if (ep->mode != HAWQ_EPI_RESIDUAL || !ep->relu || ep->y_bits != 16) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: RESIDUAL + relu + uint16 stream only");
-  if (ep->low_bits != 0 && ep->low_bits != 4 && ep->low_bits != 8) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: low_bits must be 0/4/8");
-  if (ep->low_bits) {
-    if (!out_low) return fail(HAWQ_ERR_BAD_ARG, "hawq_conv2d_dual: low_bits set but out_low is null");
-    int rc = check_me(ep->low_m, ep->low_e, "hawq_conv2d_dual low-bit copy");
-    if (rc) return rc;
-    if (!dyadic_is_fast(ep->low_m, ep->low_e)) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: low-bit ratio outside the fast range");
-  }
-  const bool ratios_one = (ep->flags & HAWQ_EP_RATIOS_LE_ONE) != 0;
-  const bool ratios_wide = !ratios_one && (ep->flags & HAWQ_EP_RATIOS_LE_2P20) != 0;
-  if (!ratios_one && !ratios_wide) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: needs a ratio-range promise (flags)");
-  const long long M = (long long)d->N * d->H * d->W;
-  if (M > 0x7fffff00ll || (long long)d2->N * d2->H * d2->W > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: too many pixels");
-  if ((M + CONV_BM - 1) / CONV_BM * (d->Cout / 64) > 0x7fffffffll)
-    return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: more than 2^31 - 1 output tiles");
+  if ((rc = check_low(__func__, ep->low_bits, ep->low_m, ep->low_e, out_low))) return rc;
+  if (ep->low_bits && !dyadic_is_fast(ep->low_m, ep->low_e)) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: low-bit ratio outside the fast range");
+  if (!(ep->flags & (HAWQ_EP_RATIOS_LE_ONE | HAWQ_EP_RATIOS_LE_2P20))) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_conv2d_dual: needs a ratio-range promise (flags)");
 
   ++g_kernel_count[4];
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.res_chan = chan2; p.out = out; p.out_low = out_low; p.status = h->status;
-  p.N = d->N; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout; p.KH = 1; p.KW = 1; p.stride = 1; p.pad = 0;
-  p.Ho = d->H; p.Wo = d->W; p.M = (int)M; p.K = d->Cin; p.cin_chunks = d->Cin / 64; p.x_pix_bytes = d->Cin * d->a_bits / 8;
-  p.mode = HAWQ_EPI_RESIDUAL; p.relu = 1; p.res_kind = 1; p.res_bits = 32; p.y_bits = 16; p.low_bits = ep->low_bits; p.low_m = ep->low_m;
-  p.low_e = ep->low_e; p.low_lo = ep->low_lo; p.low_hi = ep->low_hi;
-  p.check_ovf = 1;
-  set_bias_window(p, d->a_bits);   // main convolution only: the identity operand's bias is added with sat_add
-  p.x2 = (const uint8_t*)x2; p.w2 = w2; p.H2 = d2->H; p.W2 = d2->W; p.stride2 = d2->stride; p.cin_chunks2 = d2->Cin / 64;
-  p.x2_pix_bytes = d2->Cin * d2->a_bits / 8;
+  ConvParams p = conv_params(h, *d, x, w, chan, out);   // bias window of the main convolution only: the identity operand's bias is added with sat_add
+  const ConvParams id = conv_params(h, *d2, x2, w2, chan2, nullptr);
+  p.x2 = id.x; p.w2 = id.w; p.H2 = id.H; p.W2 = id.W; p.stride2 = id.stride; p.cin_chunks2 = id.cin_chunks; p.x2_pix_bytes = id.x_pix_bytes;
+  p.res_chan = chan2; p.out_low = out_low;
+  const hawq_epilogue_desc e = {HAWQ_EPI_RESIDUAL, 1, 0, 0, 0, 1, 32, 0, 0, 16, ep->low_bits, ep->low_m, ep->low_e, ep->low_lo, ep->low_hi, 0, ep->flags};
+  set_epilogue(p, e, true);
 
   cudaStream_t s = (cudaStream_t)stream;
   if (d->a_bits == 8) launch_conv_tail<false, true>(p, h->sm_count, s);
@@ -340,41 +370,31 @@ int hawq_linear_i8(hawq_handle* h, int32_t N, int32_t K, int32_t Cout, int32_t C
     linear_dp4a_kernel<<<grid, 256, linear_smem_bytes(K), (cudaStream_t)stream>>>(x, w, chan, fscale, out, N, K, Cout);
     return launch_check("linear_dp4a");
   }
-  hawq_conv_desc d;
-  memset(&d, 0, sizeof(d));
-  d.N = N; d.H = 1; d.W = 1; d.Cin = K; d.Cout = Cout_pad; d.kh = 1; d.kw = 1; d.stride = 1; d.pad = 0; d.a_bits = 8;
-  hawq_epilogue_desc ep;
-  memset(&ep, 0, sizeof(ep));
+  const hawq_conv_desc d = {N, 1, 1, K, Cout_pad, 1, 1, 1, 0, 8, 0};
+  hawq_epilogue_desc ep = {};
   ep.mode = HAWQ_EPI_DEQUANT_F32;
   ep.cout_store = Cout;
   return hawq_conv2d(h, &d, &ep, x, w, chan, nullptr, nullptr, fscale, out, nullptr, stream);
 }
 
 // ResNet 7x7 / 2 stem (stem.cuh): its channel set-up and requantisation policy are conv_igemm's, over K = 147 int8 products
-static ConvParams stem_params(hawq_handle* h, int N, int H, int W, const int8_t* x, const int8_t* w, const hawq_chan* chan, int clamp_lo,
-                              int clamp_hi, void* out) {
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = out; p.status = h->status;
-  p.N = N; p.H = H; p.W = W; p.Cin = 3; p.Cout = 64; p.KH = 7; p.KW = 7; p.stride = 2; p.pad = 3;
-  p.Ho = (H + 6 - 7) / 2 + 1; p.Wo = (W + 6 - 7) / 2 + 1; p.K = 147;
-  p.mode = HAWQ_EPI_REQUANT; p.relu = 1; p.lo = clamp_lo; p.hi = clamp_hi;
-  set_bias_window(p, 8);
+static ConvParams stem_params(hawq_handle* h, int N, int H, int W, const int8_t* x, const int8_t* w, const hawq_chan* chan,
+                              const hawq_epilogue_desc& ep, void* out, void* out_low) {
+  ConvParams p = conv_params(h, {N, H, W, 3, 64, 7, 7, 2, 3, 8, 0}, x, w, chan, out);
+  p.out_low = out_low;
+  set_epilogue(p, ep, true);
   return p;
 }
 
 int hawq_stem_conv_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_t* x, const int8_t* w,
                       const hawq_chan* chan, int32_t clamp_lo, int32_t clamp_hi, int16_t* out, void* stream) {
   if (!h || !x || !w || !chan || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_conv_i8: null argument");
-  if (N < 1 || H < 7 || W < 7) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_conv_i8: bad geometry");
-  if (clamp_lo < -32768 || clamp_hi > 32767 || clamp_lo > clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_conv_i8: clamp must fit int16");
+  int rc;
+  if ((rc = check_dims(__func__, N, H, W, 3, 7)) || (rc = check_clamp(__func__, clamp_lo, clamp_hi, 16))) return rc;
   if (N > 65535) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_conv_i8: N > 65535");
-  const ConvParams p = stem_params(h, N, H, W, x, w, chan, clamp_lo, clamp_hi, out);
+  const ConvParams p = stem_params(h, N, H, W, x, w, chan, {HAWQ_EPI_REQUANT, 1, 0, clamp_lo, clamp_hi}, out, nullptr);
   const dim3 grid((p.Wo + STEM_TW - 1) / STEM_TW, (p.Ho + STEM_TH - 1) / STEM_TH, N);
-  // persistent: 4 CTAs per SM loop over the tiles and stage the weights once (round-2 A/B: 0.212 -> 0.202 ms at batch 128)
-  const long long tiles = (long long)N * grid.x * grid.y;
-  const int ctas = (int)(tiles < 4LL * h->sm_count ? tiles : 4LL * h->sm_count);
-  stem_conv_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(p);
+  stem_conv_kernel<<<persistent_ctas((long long)N * grid.x * grid.y, h->sm_count), 256, 0, (cudaStream_t)stream>>>(p);
   return launch_check("stem_conv");
 }
 
@@ -383,24 +403,18 @@ int hawq_dwconv3x3(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_t C, i
                    const int8_t* w, const hawq_chan* chan, int32_t relu, int32_t out_bits, int32_t clamp_lo, int32_t clamp_hi,
                    void* out, void* stream) {
   if (!h || !x || !w || !chan || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_dwconv3x3: null argument");
-  if (N < 1 || H < 1 || W < 1 || C < 1 || (stride != 1 && stride != 2)) return fail(HAWQ_ERR_BAD_ARG, "hawq_dwconv3x3: bad geometry");
+  if (stride != 1 && stride != 2) return fail(HAWQ_ERR_BAD_ARG, "hawq_dwconv3x3: bad geometry");
+  int rc;
+  if ((rc = check_dims(__func__, N, H, W, C))) return rc;
   if (C % DW_CB != 0) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: C (%d) must be a multiple of 16", C);
   if (a_bits != 8 && a_bits != 4) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: a_bits must be 4 or 8");
   if (out_bits != 8 && out_bits != 4) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: out_bits must be 4 or 8");
-  if (clamp_lo > clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_dwconv3x3: empty clamp range");
-  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
-  const long long pix = (long long)N * H * W;
-  if (pix > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: too many pixels");
-  const long long strips = (long long)N * ((Ho + DW_ROWS - 1) / DW_ROWS) * Wo;
+  if ((rc = check_clamp(__func__, clamp_lo, clamp_hi))) return rc;
+  ConvParams p = conv_params(h, {N, H, W, C, C, 3, 3, stride, 1, a_bits, 0}, x, w, chan, out, true);
+  set_epilogue(p, {HAWQ_EPI_REQUANT, relu, out_bits, clamp_lo, clamp_hi}, true);
+  const long long strips = (long long)N * ((p.Ho + DW_ROWS - 1) / DW_ROWS) * p.Wo;
   const long long ctas = (strips + DW_THREADS - 1) / DW_THREADS * (C / DW_CB);
-  if (ctas > 0x7fffffffll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_dwconv3x3: more than 2^31 - 1 CTAs");
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = out; p.status = h->status;
-  p.N = N; p.H = H; p.W = W; p.Cin = C; p.Cout = C; p.KH = 3; p.KW = 3; p.stride = stride; p.pad = 1; p.Ho = Ho; p.Wo = Wo;
-  p.M = (int)((long long)N * Ho * Wo); p.K = 9;
-  p.mode = HAWQ_EPI_REQUANT; p.relu = relu; p.out_bits = out_bits; p.lo = clamp_lo; p.hi = clamp_hi;
-  set_bias_window(p, a_bits);
+  if ((rc = check_limits(__func__, (long long)N * H * W, ctas))) return rc;
   ++g_kernel_count[1];
   if (a_bits == 8) dwconv3x3_kernel<false><<<(unsigned)ctas, DW_THREADS, 0, (cudaStream_t)stream>>>(p);
   else dwconv3x3_kernel<true><<<(unsigned)ctas, DW_THREADS, 0, (cudaStream_t)stream>>>(p);
@@ -412,26 +426,15 @@ int hawq_stem3x3_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_
                     int32_t clamp_lo, int32_t clamp_hi, int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
                     int32_t low_lo, int32_t low_hi, void* out_low, void* stream) {
   if (!h || !x || !w || !chan || !y) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: null argument");
-  if (N < 1 || H < 1 || W < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: bad geometry");
-  if (clamp_lo > clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: empty clamp range");
-  if (y_bits == 16 && (clamp_lo < -32768 || clamp_hi > 32767)) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: clamp must fit int16");
-  if ((y_bits != 16 && y_bits != 32) || (low_bits != 0 && low_bits != 4 && low_bits != 8) || (low_bits && !out_low))
-    return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: bad output description");
-  if (low_bits) { int rc = check_me(low_m, low_e, "hawq_stem3x3_i8"); if (rc) return rc; }
-  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  if ((long long)N * H * W > 0x7fffff00ll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem3x3_i8: too many pixels");
-  const long long ctas = (long long)N * Ho * ((Wo + STEM3_PX - 1) / STEM3_PX);
-  if (ctas > 0x7fffffffll) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem3x3_i8: more than 2^31 - 1 CTAs");
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = (const uint8_t*)x; p.w = w; p.chan = chan; p.out = y; p.out_low = out_low; p.status = h->status;
-  p.N = N; p.H = H; p.W = W; p.Cin = 3; p.Cout = 64; p.KH = 3; p.KW = 3; p.stride = 2; p.pad = 1; p.Ho = Ho; p.Wo = Wo;
-  p.M = (int)((long long)N * Ho * Wo); p.K = 27;
-  p.mode = HAWQ_EPI_REQUANT; p.relu = relu; p.lo = clamp_lo; p.hi = clamp_hi; p.y_bits = y_bits;
-  p.low_bits = low_bits; p.low_m = low_m; p.low_e = low_e; p.low_lo = low_lo; p.low_hi = low_hi;
-  // a low-bit ratio > 1 takes the CTA to the exact requantisation (load_channel_block)
-  p.scalar_over_one = p.scalar_unchecked = low_bits != 0 && !dyadic_is_fast(low_m, low_e);
-  set_bias_window(p, 8);
+  int rc;
+  if ((rc = check_dims(__func__, N, H, W, 3)) || (rc = check_clamp(__func__, clamp_lo, clamp_hi, y_bits == 16 ? 16 : 0))) return rc;
+  if (y_bits != 16 && y_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem3x3_i8: y_bits must be 16/32");
+  if ((rc = check_low(__func__, low_bits, low_m, low_e, out_low))) return rc;
+  ConvParams p = conv_params(h, {N, H, W, 3, 64, 3, 3, 2, 1, 8, 0}, x, w, chan, y);
+  p.out_low = out_low;
+  set_epilogue(p, {HAWQ_EPI_REQUANT, relu, 0, clamp_lo, clamp_hi, 0, 0, 0, 0, y_bits, low_bits, low_m, low_e, low_lo, low_hi}, true);
+  const long long ctas = (long long)N * p.Ho * ((p.Wo + STEM3_PX - 1) / STEM3_PX);
+  if ((rc = check_limits(__func__, (long long)N * H * W, ctas))) return rc;
   ++g_kernel_count[2];
   stem3x3_kernel<<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(p);
   return launch_check("stem3x3");
@@ -441,21 +444,19 @@ int hawq_stem_pool_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int
                       int32_t clamp_lo, int32_t clamp_hi, int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
                       int32_t low_lo, int32_t low_hi, void* out_low, void* stream) {
   if (!h || !x || !w256 || !chan || !y) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_pool_i8: null argument");
-  if (N < 1 || H < 7 || W < 7) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_pool_i8: bad geometry");
-  if (clamp_lo < -32768 || clamp_hi > 32767 || clamp_lo > clamp_hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_pool_i8: clamp must fit int16");
-  if ((y_bits != 16 && y_bits != 32) || (low_bits != 0 && low_bits != 4 && low_bits != 8) || (low_bits && !out_low))
-    return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_pool_i8: bad output description");
-  if (low_bits) { int rc = check_me(low_m, low_e, "hawq_stem_pool_i8"); if (rc) return rc; }
+  int rc;
+  if ((rc = check_dims(__func__, N, H, W, 3, 7)) || (rc = check_clamp(__func__, clamp_lo, clamp_hi, 16))) return rc;
+  if (y_bits != 16 && y_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "hawq_stem_pool_i8: y_bits must be 16/32");
+  if ((rc = check_low(__func__, low_bits, low_m, low_e, out_low))) return rc;
   if (W % 16 != 0 || W > 256 || (low_bits && !dyadic_is_fast(low_m, low_e)))
     return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_pool_i8: shape / ratio outside the fused kernel (use hawq_stem_conv_i8 + hawq_maxpool_requant)");
   if (N > 65535) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_stem_pool_i8: N > 65535");
-  ConvParams p = stem_params(h, N, H, W, x, w256, chan, clamp_lo, clamp_hi, y);
-  p.y_bits = y_bits; p.low_bits = low_bits; p.low_m = low_m; p.low_e = low_e; p.low_lo = low_lo; p.low_hi = low_hi; p.out_low = out_low;
-  const int Po = (p.Ho + 2 - 3) / 2 + 1, Qo = (p.Wo + 2 - 3) / 2 + 1;
+  const ConvParams p = stem_params(h, N, H, W, x, w256, chan,
+                                   {HAWQ_EPI_REQUANT, 1, 0, clamp_lo, clamp_hi, 0, 0, 0, 0, y_bits, low_bits, low_m, low_e, low_lo, low_hi}, y, out_low);
+  const int Po = out_size(p.Ho, 3, 2, 1), Qo = out_size(p.Wo, 3, 2, 1);
   const long long tiles = (long long)N * ((Po + STEMP_PH - 1) / STEMP_PH) * ((Qo + STEMP_PW - 1) / STEMP_PW);
-  const int ctas = (int)(tiles < 4LL * h->sm_count ? tiles : 4LL * h->sm_count);
   ++g_kernel_count[6];
-  stem_pool_kernel<<<ctas, 256, 0, (cudaStream_t)stream>>>(p);
+  stem_pool_kernel<<<persistent_ctas(tiles, h->sm_count), 256, 0, (cudaStream_t)stream>>>(p);
   return launch_check("stem_pool");
 }
 
@@ -465,9 +466,9 @@ int hawq_maxpool_requant(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_
   if (!h || !x) return fail(HAWQ_ERR_BAD_ARG, "hawq_maxpool_requant: null argument");
   if (C % 8 != 0) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_maxpool_requant: C %% 8 != 0");
   if ((y_bits != 0 && y_bits != 16 && y_bits != 32) || (y_bits && !y)) return fail(HAWQ_ERR_BAD_ARG, "hawq_maxpool_requant: bad y");
-  if ((low_bits != 0 && low_bits != 4 && low_bits != 8) || (low_bits && !out_low)) return fail(HAWQ_ERR_BAD_ARG, "hawq_maxpool_requant: bad low");
-  if (low_bits) { int rc = check_me(low_m, low_e, "hawq_maxpool_requant"); if (rc) return rc; }
-  const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
+  int rc;
+  if ((rc = check_low(__func__, low_bits, low_m, low_e, out_low)) || (rc = check_dims(__func__, N, H, W, C))) return rc;
+  const int Ho = out_size(H, 3, 2, 1), Wo = out_size(W, 3, 2, 1);
   const long long total = (long long)N * Ho * Wo * (C / 8);
   maxpool_requant_kernel<<<grid_for(total, h->sm_count), 256, 0, (cudaStream_t)stream>>>(
       x, N, H, W, C, Ho, Wo, y_bits, y, low_bits, low_m, low_e, low_lo, low_hi, out_low);
@@ -478,9 +479,8 @@ int hawq_avgpool_requant(hawq_handle* h, int32_t N, int32_t HW, int32_t C, int32
                          int32_t e, int32_t lo, int32_t hi, int8_t* out, void* stream) {
   if (!h || !x || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_avgpool_requant: null argument");
   if (x_bits != 16 && x_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "hawq_avgpool_requant: x_bits must be 16/32");
-  if (lo < -128 || hi > 127) return fail(HAWQ_ERR_BAD_ARG, "hawq_avgpool_requant: clamp must fit int8");
-  int rc = check_me(m, e, "hawq_avgpool_requant");
-  if (rc) return rc;
+  int rc;
+  if ((rc = check_clamp(__func__, lo, hi, 8)) || (rc = check_me(__func__, "requant", m, e)) || (rc = check_dims(__func__, N, HW, 1, C))) return rc;
   avgpool_requant_kernel<<<grid_for((long long)N * C, h->sm_count), 256, 0, (cudaStream_t)stream>>>(x, N, HW, C, x_bits, m, e, lo, hi, out);
   return launch_check("avgpool_requant");
 }
@@ -489,7 +489,7 @@ int hawq_quantize_input_f32(hawq_handle* h, int32_t N, int32_t C, int32_t H, int
                             int32_t lo, int32_t hi, int8_t* out, void* stream) {
   if (!h || !x || !out) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_f32: null argument");
   if (!(scale > 0.f)) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_f32: scale must be > 0");
-  if (lo < -128 || hi > 127) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_f32: clamp must fit int8");
+  if (int rc = check_clamp("hawq_quantize_input_f32", lo, hi, 8)) return rc;
   const float inv = 1.0f / scale;  // fp32 division, as `1. / scale` in linear_quantize (quant_utils.py:97)
   quantize_input_kernel<<<grid_for((long long)N * H * W, h->sm_count), 256, 0, (cudaStream_t)stream>>>(x, N, C, H, W, inv, lo, hi, out);
   return launch_check("quantize_input");
@@ -498,9 +498,10 @@ int hawq_quantize_input_f32(hawq_handle* h, int32_t N, int32_t C, int32_t H, int
 int hawq_quantize_input_u8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const uint8_t* x, const float* mean3,
                            const float* std3, float scale, int32_t lo, int32_t hi, int8_t* out, void* stream) {
   if (!h || !x || !out || !mean3 || !std3) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_u8: null argument");
-  if (N < 1 || H < 1 || W < 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_u8: empty shape");
+  int rc;
+  if ((rc = check_dims(__func__, N, H, W, 3))) return rc;
   if (!(scale > 0.f)) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_u8: scale must be > 0");
-  if (lo < -128 || hi > 127 || lo > hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_u8: clamp must fit int8");
+  if ((rc = check_clamp(__func__, lo, hi, 8))) return rc;
   for (int c = 0; c < 3; ++c)
     if (!(std3[c] > 0.f)) return fail(HAWQ_ERR_BAD_ARG, "hawq_quantize_input_u8: std must be > 0");
   const float inv = 1.0f / scale;  // fp32 division, as `1. / scale` in linear_quantize (quant_utils.py:97)
@@ -520,7 +521,7 @@ int hawq_resize_crop_quantize_u8(hawq_handle* h, int32_t B, const uint8_t* pixel
     return fail(HAWQ_ERR_UNSUPPORTED, "hawq_resize_crop_quantize_u8: resize %d must lie in %d..%d and cover the crop %dx%d", S,
                 ET_MIN_RESIZE, ET_MAX_SIDE, Ch, Cw);
   if (!(scale > 0.f)) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: scale must be > 0");
-  if (lo < -128 || hi > 127 || lo > hi) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: clamp must fit int8");
+  if (int rc = check_clamp("hawq_resize_crop_quantize_u8", lo, hi, 8)) return rc;
   for (int c = 0; c < 3; ++c)
     if (!(std3[c] > 0.f)) return fail(HAWQ_ERR_BAD_ARG, "hawq_resize_crop_quantize_u8: std must be > 0");
   const float inv = 1.0f / scale;  // as hawq_quantize_input_u8
@@ -537,6 +538,7 @@ int hawq_requant(hawq_handle* h, int64_t rows, int32_t C, int32_t x_bits, const 
   if (x_bits != 16 && x_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "hawq_requant: x_bits must be 16/32");
   if (out_bits != 4 && out_bits != 8 && out_bits != 16 && out_bits != 32) return fail(HAWQ_ERR_BAD_ARG, "hawq_requant: out_bits must be 4/8/16/32");
   if (chan_stride != 0 && chan_stride != 1) return fail(HAWQ_ERR_BAD_ARG, "hawq_requant: chan_stride must be 0/1");
+  if (int rc = check_clamp("hawq_requant", lo, hi)) return rc;
   requant_kernel<<<grid_for(rows * (C / 8), h->sm_count), 256, 0, (cudaStream_t)stream>>>(x, rows, C, x_bits, chan, chan_stride, relu, out_bits, lo, hi, out);
   return launch_check("requant");
 }
@@ -546,10 +548,7 @@ int hawq_add_requant(hawq_handle* h, int64_t rows, int32_t C, const int32_t* acc
                      void* stream) {
   if (!h || !acc || !chan || !ep || !res) return fail(HAWQ_ERR_BAD_ARG, "hawq_add_requant: null argument");
   if (C % 8 != 0) return fail(HAWQ_ERR_UNSUPPORTED, "hawq_add_requant: C %% 8 != 0");
-  if (ep->res_kind == 1 && !res_chan) return fail(HAWQ_ERR_BAD_ARG, "hawq_add_requant: res_kind 1 needs res_chan");
-  if (ep->res_kind == 0) { int rc = check_me(ep->res_m, ep->res_e, "hawq_add_requant"); if (rc) return rc; }
-  if (ep->y_bits == 16 && !ep->relu) return fail(HAWQ_ERR_BAD_ARG, "hawq_add_requant: uint16 residual stream requires relu");
-  if ((ep->y_bits && !y) || (ep->low_bits && !out_low)) return fail(HAWQ_ERR_BAD_ARG, "hawq_add_requant: missing output");
+  if (int rc = check_residual("hawq_add_requant", ep, res, res_chan, y, out_low)) return rc;
   AddRequantParams p;
   p.acc = acc; p.chan = chan; p.res = res; p.res_chan = res_chan; p.y = y; p.out_low = out_low; p.status = h->status;
   p.rows = rows; p.C = C; p.relu = ep->relu; p.res_kind = ep->res_kind; p.res_bits = ep->res_bits; p.res_m = ep->res_m;

@@ -184,7 +184,9 @@ int hawq_stem_pool_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int
 /* nn.MaxPool2d(3,2,1) (q_resnet.py:119) on the int16 stem output + the first unit's quant_act (case 0, scalar m,e).
  * Precondition: 0 <= x <= 32767 (the post-ReLU stem output); the kernel pads with 0 and reads the maxima as unsigned, so
  * negative inputs give unspecified results.
- * y: residual stream (y_bits 16 -> uint16, 32 -> int32); out_low: int8 / packed u4 (low_bits 8 / 4, 0 = none). */
+ * y: residual stream (y_bits 16 -> uint16, 32 -> int32); out_low: int8 / packed u4 (low_bits 8 / 4, 0 = none).
+ * Requires N, H, W, C >= 1, y_bits 0 / 16 / 32, low_bits 0 / 4 / 8 (1 <= low_e <= 62, low_m <= 2^31) and C % 8 == 0 (else
+ * HAWQ_ERR_UNSUPPORTED); a call outside these returns HAWQ_ERR_BAD_ARG and launches nothing. */
 int hawq_maxpool_requant(hawq_handle* h, int32_t N, int32_t H, int32_t W, int32_t C, const int16_t* x,
                          int32_t y_bits, void* y, int32_t low_bits, uint32_t low_m, int32_t low_e,
                          int32_t low_lo, int32_t low_hi, void* out_low, void* stream);
@@ -206,14 +208,16 @@ int hawq_stem3x3_i8(hawq_handle* h, int32_t N, int32_t H, int32_t W, const int8_
                     int32_t low_lo, int32_t low_hi, void* out_low, void* stream);
 
 /* QuantAveragePool2d (quant_modules.py:585-602) + quant_act_output (q_resnet.py:131): x residual stream
- * [N,HW,C] (x_bits 16/32) -> int8 [N,C] = clamp(RHE(trunc_avg(x) * m / 2^e)). */
+ * [N,HW,C] (x_bits 16/32) -> int8 [N,C] = clamp(RHE(trunc_avg(x) * m / 2^e)).
+ * Requires N, HW, C >= 1, -128 <= lo <= hi <= 127, 1 <= e <= 62 and m <= 2^31; otherwise HAWQ_ERR_BAD_ARG (nothing launched). */
 int hawq_avgpool_requant(hawq_handle* h, int32_t N, int32_t HW, int32_t C, int32_t x_bits, const void* x,
                          uint32_t m, int32_t e, int32_t lo, int32_t hi, int8_t* out, void* stream);
 
 /* ---- stand-alone (unfused) pieces of the module API --------------------------------------------------------- */
 /* QuantAct input branch (quant_modules.py:271-274): q = clamp(round((1/scale) * x)), fp32 RNE.
  * x fp32 NCHW [N,C,H,W] -> int8 NHWC [N,H,W,C].  +-inf clamp to lo / hi.  NaN is outside the reference's semantics (its
- * integer cast of NaN is undefined): the result for a NaN element is unspecified. */
+ * integer cast of NaN is undefined): the result for a NaN element is unspecified.  Requires scale > 0 and -128 <= lo <= hi <= 127
+ * (else HAWQ_ERR_BAD_ARG, nothing launched). */
 int hawq_quantize_input_f32(hawq_handle* h, int32_t N, int32_t C, int32_t H, int32_t W, const float* x,
                             float scale, int32_t lo, int32_t hi, int8_t* out, void* stream);
 /* uint8 image entry (tvm_benchmark/test_resnet_accuracy_imagenet.py:62-75 quantize_image after transforms.ToTensor + Normalize
@@ -239,10 +243,14 @@ int hawq_resize_crop_quantize_u8(hawq_handle* h, int32_t B, const uint8_t* pixel
                                  int32_t S, int32_t Ch, int32_t Cw, const float* mean3, const float* std3, float scale, int32_t lo,
                                  int32_t hi, int8_t* out, void* stream);
 /* fixedpoint_fn case 0 stand-alone (QuantAct after a conv or at unit entry): x [rows,C] (x_bits 16 = uint16 residual,
- * 32 = int32), per-channel chan (bias is added; pass 0) or scalar when chan_stride == 0 (chan[0] used for all). */
+ * 32 = int32), per-channel chan (bias is added; pass 0) or scalar when chan_stride == 0 (chan[0] used for all).
+ * Requires lo <= hi (else HAWQ_ERR_BAD_ARG, nothing launched) and C % 8 == 0 (else HAWQ_ERR_UNSUPPORTED). */
 int hawq_requant(hawq_handle* h, int64_t rows, int32_t C, int32_t x_bits, const void* x, const hawq_chan* chan,
                  int32_t chan_stride, int32_t relu, int32_t out_bits, int32_t lo, int32_t hi, void* out, void* stream);
-/* fixedpoint_fn case 1 stand-alone: y = [relu](RHE(res*m1/2^e1) + RHE((acc+bias)*m/2^e)); same operands as the fused form. */
+/* fixedpoint_fn case 1 stand-alone: y = [relu](RHE(res*m1/2^e1) + RHE((acc+bias)*m/2^e)); same operands as the fused form, checked
+ * by the same rules as a RESIDUAL hawq_conv2d: res_kind 0 (res_bits 16 / 32, 1 <= res_e <= 62, res_m <= 2^31) or 1 (res_chan),
+ * y_bits 0 / 16 / 32 (16 needs relu), low_bits 0 / 4 / 8 (the same range for low_m, low_e), at least one output; otherwise
+ * HAWQ_ERR_BAD_ARG (nothing launched).  C % 8 != 0 returns HAWQ_ERR_UNSUPPORTED. */
 int hawq_add_requant(hawq_handle* h, int64_t rows, int32_t C, const int32_t* acc, const hawq_chan* chan,
                      const hawq_epilogue_desc* ep, const void* res, const hawq_chan* res_chan,
                      void* y, void* out_low, void* stream);
