@@ -8,6 +8,7 @@ Public surface (mirrors the reference's module API for the quantized forward pat
   bit_config   bit_config_dict(), get_bit_config(arch, scheme), stamp_bit_config(model, cfg)
   engine       compile_model(model, example) -> CompiledModel (one CUDA graph per GPU), all_gather_logits
   eval_transform  PackedImages, collate_images: ragged batches of decoded images for compile_model(..., resize=256)
+  engine_file  CompiledModel.save(path) -> one plan file; load_engine(path) runs it on the library's runtime, without the model
   ops / _lib   the C ABI (include/hawq_b200.h) through ctypes
 The frozen path runs only on the in-tree CUDA library (sm_90a); there is no CPU or PyTorch fallback.
 """
@@ -18,6 +19,7 @@ from .q_resnet import (Q_ResBlockBn, Q_ResNet18, Q_ResNet50, Q_ResNet101, Q_ResU
 from .q_mobilenetv2 import Q_LinearBottleneck, Q_MobileNetV2, q_mobilenetv2_w1  # noqa: F401
 from .bit_config import bit_config_dict, get_bit_config, stamp_bit_config  # noqa: F401
 from .engine import CompiledModel, all_gather_logits, compile_model, shard_range  # noqa: F401
+from .engine_file import LoadedEngine, load_engine  # noqa: F401
 from .eval_transform import PackedImages, collate_images  # noqa: F401
 from .qtensor import IntActivation  # noqa: F401
 from .checkpoint import (apply_integer_checkpoint, export_tvm_params, load_quantized_checkpoint,  # noqa: F401

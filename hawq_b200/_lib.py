@@ -44,7 +44,20 @@ FLAG_BAD_RATIO = 2
 FLAG_REQUANT_OVERFLOW = 4
 EP_RATIOS_LE_ONE = 1
 EP_RATIOS_LE_2P20 = 2
-ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_CUDA = -1, -2, -3   # hawq_status
+ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_CUDA, ERR_RESULT_INVALID = -1, -2, -3, -4   # hawq_status
+
+
+class hawq_engine_info(C.Structure):
+    _fields_ = [("input_dtype", C.c_int32), ("residual_bits", C.c_int32), ("input_shape", C.c_int64 * 4), ("input_bytes", C.c_int64),
+                ("output_shape", C.c_int64 * 2), ("arena_bytes", C.c_int64), ("constant_bytes", C.c_int64), ("launches", C.c_int64 * 3),
+                ("fallbacks", C.c_int64)]
+
+
+# enum hawq_engine_entry: the entry id of each entry point in a plan file is its index here
+ENGINE_ENTRIES = ("hawq_conv2d", "hawq_conv2d_dual", "hawq_linear_i8", "hawq_stem_conv_i8", "hawq_stem_pool_i8", "hawq_dwconv3x3",
+                  "hawq_stem3x3_i8", "hawq_maxpool_requant", "hawq_avgpool_requant", "hawq_quantize_input_f32", "hawq_quantize_input_u8",
+                  "hawq_resize_crop_quantize_u8", "hawq_requant", "hawq_add_requant", "hawq_dequant_f32", "hawq_pack_i4", "hawq_unpack_i4")
+ENGINE_FORMAT = 1
 
 _vp, _i32, _i64, _u32, _f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float
 _conv_args = [_vp, C.POINTER(hawq_conv_desc), C.POINTER(hawq_epilogue_desc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
@@ -86,6 +99,15 @@ SIGNATURES = {
     "hawq_retile_weights": (_i32, [_vp, _vp, _i32, _i64, _vp, _vp]),
     "hawq_debug_kernel_count": (_i64, [_i32]),
     "hawq_workspace_bytes": (_i64, [C.POINTER(hawq_conv_desc), C.POINTER(hawq_epilogue_desc)]),
+    "hawq_engine_check": (_i32, [_vp, _i64, C.POINTER(hawq_engine_info)]),
+    "hawq_engine_load": (_i32, [_i32, _vp, _i64, C.POINTER(_vp)]),
+    "hawq_engine_destroy": (_i32, [_vp]),
+    "hawq_engine_input": (_vp, [_vp]),
+    "hawq_engine_output": (_vp, [_vp]),
+    "hawq_engine_get_info": (_i32, [_vp, C.POINTER(hawq_engine_info)]),
+    "hawq_engine_enqueue": (_i32, [_vp, _vp]),
+    "hawq_engine_status": (_i32, [_vp, C.POINTER(_i32)]),
+    "hawq_engine_run": (_i32, [_vp, _vp, C.POINTER(_i32)]),
 }
 
 _lib = None

@@ -121,3 +121,29 @@ def build_library(force=False, verbose=False, extra_flags=()):
         finally:
             fcntl.flock(lock, fcntl.LOCK_UN)
     return OUT
+
+
+RUNNER_SRC = os.path.join(os.path.dirname(_HERE), "tools", "hawq_run.c")
+RUNNER = os.path.join(_HERE, "hawq_run")
+
+
+def _cuda_root():
+    return os.path.dirname(os.path.dirname(os.path.realpath(_nvcc())))
+
+
+def build_runner(verbose=False):
+    """Compile tools/hawq_run.c next to the library: the standalone runner of plan files.  It links libhawq_b200.so (found next to
+    the binary) and the static CUDA runtime, and nothing of Python or torch."""
+    cuda = _cuda_root()
+    tmp = "%s.tmp.%d" % (RUNNER, os.getpid())
+    cmd = ["gcc", "-O2", "-std=c11", "-Wall", "-I", INCLUDE, "-I", os.path.join(cuda, "include"), "-o", tmp, RUNNER_SRC, "-L", _HERE,
+           "-l:libhawq_b200.so", "-Wl,-rpath,$ORIGIN", "-L", os.path.join(cuda, "lib64"), "-lcudart_static", "-lrt", "-lpthread", "-ldl"]
+    if verbose:
+        print(" ".join(cmd).replace(tmp, RUNNER))
+    r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    if r.returncode != 0:
+        if os.path.exists(tmp):
+            os.remove(tmp)
+        raise RuntimeError("building hawq_run failed:\n" + r.stdout)
+    os.replace(tmp, RUNNER)
+    return RUNNER

@@ -25,13 +25,16 @@ struct hawq_handle {
 static thread_local char g_err[512] = "";
 static long long g_kernel_count[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // hawq_debug_kernel_count: launches by kernel family (not atomic: debugging aid)
 
-static int fail(int code, const char* fmt, ...) {
+// Sets the thread's hawq_last_error message and returns code; engine_file.cu reports through it too
+namespace hawq {
+int fail(int code, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
   return code;
 }
+}  // namespace hawq
 
 #define CUDA_TRY(expr)                                                                         \
   do {                                                                                         \

@@ -331,6 +331,14 @@ class CompiledModel:
     def gpu_launches(self):
         return self.launches.get(self.residual_bits, 0)
 
+    def save(self, path):
+        """Write this engine as one plan file (engine_file.py): its fast, int32 and safe forwards, recorded launch by launch, with
+        the weights and tables they read.  ``hawq_b200.load_engine`` or the C runtime (include/hawq_b200.h) runs it without the model.
+        Builds the fallback graphs not built yet.  Not for ``resize`` or ``gather`` engines (NotImplementedError).  Returns the
+        file's size in bytes."""
+        from . import engine_file
+        return engine_file.save(self, path)
+
 
 def compile_model(model, example, use_cuda_graph=True, residual_bits=16, mean=IMAGENET_MEAN, std=IMAGENET_STD, gather=False, group=None,
                   resize=None):

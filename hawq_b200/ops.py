@@ -86,11 +86,52 @@ def _ctx(t):
     return handle(idx), C.c_void_p(torch.cuda.current_stream(idx).cuda_stream)
 
 
+class _Ptr(C.c_void_p):
+    """The device pointer of a tensor while this thread records launches (``recording``), with its storage's (base, bytes)."""
+
+
 def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
+    if t is None:
+        return None
+    if getattr(_local, "recorder", None) is None:
+        return C.c_void_p(t.data_ptr())
+    p = _Ptr(t.data_ptr())
+    s = t.untyped_storage()
+    p.storage = (s.data_ptr(), s.nbytes())
+    return p
 
 
 timer = None   # set to a list to record (kernel, info, start_event, end_event) per launch (bench.py roofline leg)
+
+
+@contextlib.contextmanager
+def recording():
+    """Every launch this thread makes inside the block is appended to the yielded list as (entry point, arguments) (engine_file.py
+    turns them into a plan file).  An argument is ("i32" | "u32" | "i64" | "f32", value), ("null",), ("ptr", address, storage base,
+    storage bytes) (base and bytes None when the pointer did not come from a tensor), or ("blob", bytes) for a struct or array passed by
+    pointer, by value.  The handle and the stream are implicit."""
+    saved = getattr(_local, "recorder", None)
+    _local.recorder = rec = []
+    try:
+        yield rec
+    finally:
+        _local.recorder = saved
+
+
+_ARG_KINDS = {_lib._i32: "i32", _lib._u32: "u32", _lib._i64: "i64", _lib._f32: "f32"}
+
+
+def _recorded(fn, args):
+    out = []
+    for a, ctype in zip(args, _lib.SIGNATURES[fn][1][1:-1]):
+        if ctype is C.c_void_p:
+            v = a.value if isinstance(a, C.c_void_p) else a
+            out.append(("null",) if v is None else ("ptr", v) + getattr(a, "storage", (None, None)))
+        elif ctype in _ARG_KINDS:
+            out.append((_ARG_KINDS[ctype], a.value if isinstance(a, C._SimpleCData) else a))
+        else:
+            out.append(("blob", bytes(getattr(a, "_obj", a))))
+    return fn, out
 
 
 def _launch(t, fn, *args, label=None, work=None):
@@ -103,6 +144,9 @@ def _launch(t, fn, *args, label=None, work=None):
         ev0.record()
     _lib.check(getattr(_lib.load(), fn)(h, *args, s))
     _local.launches = thread_launch_count() + 1
+    rec = getattr(_local, "recorder", None)
+    if rec is not None:
+        rec.append(_recorded(fn, args))
     if ev0 is not None:
         info = work()
         ev1 = torch.cuda.Event(enable_timing=True)

@@ -47,7 +47,8 @@ enum hawq_status {
   HAWQ_OK = 0,
   HAWQ_ERR_BAD_ARG = -1,      /* null pointer, non-positive size, inconsistent descriptor */
   HAWQ_ERR_UNSUPPORTED = -2,  /* shape / bit-width combination this build has no kernel for */
-  HAWQ_ERR_CUDA = -3          /* CUDA runtime error (message in hawq_last_error) */
+  HAWQ_ERR_CUDA = -3,         /* CUDA runtime error (message in hawq_last_error) */
+  HAWQ_ERR_RESULT_INVALID = -4 /* hawq_engine_run: HAWQ_FLAG_BAD_RATIO was raised, the logits are invalid */
 };
 
 /* bits of the device status word */
@@ -281,6 +282,92 @@ int hawq_retile_weights(hawq_handle* h, const int8_t* w_ohwi, int32_t Cout, int6
 int64_t hawq_debug_kernel_count(int32_t family);
 /* workspace query kept for ABI completeness: this build needs no scratch beyond caller tensors */
 int64_t hawq_workspace_bytes(const hawq_conv_desc* d, const hawq_epilogue_desc* ep);
+
+/* ---- engine files: a compiled forward saved to one file and replayed without Python (INTEGRATION.md §3) ------------ */
+/* A plan file (CompiledModel.save) holds every launch of one forward as (entry id, arguments), for three sequences: "fast" (the
+ * engine's residual stream width, ratio promises), "int32" (the fallback when the uint16 stream overflowed; absent when the fast
+ * sequence already stores int32) and "safe" (no ratio promises: the fallback after HAWQ_FLAG_REQUANT_OVERFLOW).  Every pointer
+ * argument is an offset into one of four regions: the input binding, the output binding (fp32 logits [N, classes], shared by the
+ * three sequences), the constants (weights and per-channel tables, stored in the file) and the arena (every other buffer, laid out
+ * with the aliasing of the recorded run; zeroed at load).  The loader captures each sequence into a CUDA graph that calls the entry
+ * points of this header with exactly the recorded arguments, so a replay runs the same kernels on the same integers.
+ *
+ * Format (little-endian, fixed-width fields):
+ *   header, 40 bytes: "HAWQPLAN", u32 format version (HAWQ_ENGINE_FORMAT), u32 HAWQ_ABI_VERSION, u32 compute capability major (9)
+ *     and minor (0), u64 body bytes, u32 CRC-32 (zlib's) of the body, u32 zero;
+ *   body: u32 input dtype (hawq_engine_dtype), u32 residual bits of the fast sequence (16 / 32), i64 input shape[4], i64 input bytes;
+ *     i64 output shape[2]; u64 constant bytes, the constants; u64 arena bytes; u32 sequence count, then per sequence u32 kind
+ *     (hawq_engine_seq), u32 record count, and per record u16 entry id (hawq_engine_entry), u16 argument count and the arguments
+ *     in the entry's order without handle and stream, each a u8 kind (hawq_engine_arg) and its value: i32 / u32 / f32 4 bytes,
+ *     i64 8 bytes, null nothing, ptr a u8 region (hawq_engine_region) and a u64 offset, blob a u32 length and the bytes (the value
+ *     of a hawq_conv_desc, a hawq_epilogue_desc or a float[3] passed by pointer).
+ * Trust: a plan file is trusted like a shared library.  Its structure is validated, its launches are not: the extents that a
+ * descriptor determines are checked only by each entry point's own argument checks. */
+#define HAWQ_ENGINE_FORMAT 1
+
+/* entry ids of a plan file: the entry points a recorded forward launches */
+enum hawq_engine_entry {
+  HAWQ_ENTRY_CONV2D = 0,
+  HAWQ_ENTRY_CONV2D_DUAL = 1,
+  HAWQ_ENTRY_LINEAR_I8 = 2,
+  HAWQ_ENTRY_STEM_CONV_I8 = 3,
+  HAWQ_ENTRY_STEM_POOL_I8 = 4,
+  HAWQ_ENTRY_DWCONV3X3 = 5,
+  HAWQ_ENTRY_STEM3X3_I8 = 6,
+  HAWQ_ENTRY_MAXPOOL_REQUANT = 7,
+  HAWQ_ENTRY_AVGPOOL_REQUANT = 8,
+  HAWQ_ENTRY_QUANTIZE_INPUT_F32 = 9,
+  HAWQ_ENTRY_QUANTIZE_INPUT_U8 = 10,
+  HAWQ_ENTRY_RESIZE_CROP_QUANTIZE_U8 = 11,
+  HAWQ_ENTRY_REQUANT = 12,
+  HAWQ_ENTRY_ADD_REQUANT = 13,
+  HAWQ_ENTRY_DEQUANT_F32 = 14,
+  HAWQ_ENTRY_PACK_I4 = 15,
+  HAWQ_ENTRY_UNPACK_I4 = 16,
+  HAWQ_ENTRY_COUNT = 17
+};
+enum hawq_engine_arg { HAWQ_ARG_I32 = 1, HAWQ_ARG_U32 = 2, HAWQ_ARG_I64 = 3, HAWQ_ARG_F32 = 4, HAWQ_ARG_NULL = 5, HAWQ_ARG_PTR = 6, HAWQ_ARG_BLOB = 7 };
+enum hawq_engine_region { HAWQ_REGION_INPUT = 0, HAWQ_REGION_OUTPUT = 1, HAWQ_REGION_CONST = 2, HAWQ_REGION_ARENA = 3 };
+enum hawq_engine_seq { HAWQ_SEQ_FAST = 0, HAWQ_SEQ_INT32 = 1, HAWQ_SEQ_SAFE = 2 };
+/* input binding: int8 NHWC (already quantised), uint8 NHWC pixels, or fp32 NCHW (normalised) */
+enum hawq_engine_dtype { HAWQ_DTYPE_INT8 = 0, HAWQ_DTYPE_UINT8 = 1, HAWQ_DTYPE_FLOAT32 = 2 };
+
+typedef struct hawq_engine hawq_engine;
+
+typedef struct {
+  int32_t input_dtype;      /* hawq_engine_dtype */
+  int32_t residual_bits;    /* of the fast sequence: 16 (an int32 sequence follows an overflow) or 32 */
+  int64_t input_shape[4];
+  int64_t input_bytes;
+  int64_t output_shape[2];  /* fp32 [N, classes] */
+  int64_t arena_bytes;
+  int64_t constant_bytes;
+  int64_t launches[3];      /* entry-point calls per sequence (hawq_engine_seq); 0: the sequence is absent */
+  int64_t fallbacks;        /* a loaded engine: hawq_engine_run calls that replayed the int32 or safe sequence */
+} hawq_engine_info;
+
+/* Parses and validates a whole plan file in host memory without touching a device: magic, versions, checksum, every section and
+ * record inside the buffer, entry ids and argument kinds and counts against each entry's signature, every ptr offset inside its
+ * region.  HAWQ_ERR_BAD_ARG with a message on any failure; on success fills info (fallbacks 0) when info is not null. */
+int hawq_engine_check(const void* data, int64_t bytes, hawq_engine_info* info);
+/* Checks the file, creates the engine's own handle (its own status word) on `device`, allocates the regions, uploads the constants,
+ * zeroes the arena and captures each sequence into a CUDA graph on a private stream.  The caller's current device is unchanged. */
+int hawq_engine_load(int device, const void* data, int64_t bytes, hawq_engine** out);
+/* frees everything the engine owns (synchronises its device) */
+int hawq_engine_destroy(hawq_engine* eng);
+/* device pointers of the input binding (input_bytes) and the output binding (fp32 [N, classes]) */
+void* hawq_engine_input(const hawq_engine* eng);
+float* hawq_engine_output(const hawq_engine* eng);
+int hawq_engine_get_info(const hawq_engine* eng, hawq_engine_info* info);
+/* resets the status word and replays the fast sequence on `stream`; the word is copied to a host-readable word at its end.  No host
+ * synchronisation and no check: read the word with hawq_engine_status once the stream is synchronised */
+int hawq_engine_enqueue(hawq_engine* eng, void* stream);
+int hawq_engine_status(const hawq_engine* eng, int32_t* flags);
+/* The exact forward: replays the fast sequence, synchronises `stream` and reads the status word (into *flags when not null).
+ * HAWQ_FLAG_BAD_RATIO: returns HAWQ_ERR_RESULT_INVALID.  HAWQ_FLAG_REQUANT_OVERFLOW: replays the safe sequence.  Otherwise, with a
+ * 16-bit fast sequence, HAWQ_FLAG_RESIDUAL_OVERFLOW replays the int32 sequence.  A fallback replay is enqueued on `stream` after
+ * the fast one and counted in hawq_engine_info.fallbacks; the output binding holds the exact logits once `stream` reaches it. */
+int hawq_engine_run(hawq_engine* eng, void* stream, int32_t* flags);
 
 #ifdef __cplusplus
 }
